@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- MSDeformAttn hot-path benchmark (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- MSDeformAttn hot-path benchmark (BASELINE.json metric) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -10,7 +10,7 @@ One *step* = one pass of the hot path over one batch of the workload (default cf
 COCO-shape 1333x800, R50 4-level features, 300 queries, 8 heads x 32, 4 levels x 4 points, batch 2, fp32): the
 6 encoder-shaped + 6 decoder-shaped MSDeformAttn calls of one transformer pass, each forward AND backward,
 through the reference-facing module functions (``MultiScaleDeformableAttention.ms_deform_attn_forward/backward``
--> C ABI).  Every call has its own input tensors (12 distinct sets, ~1 GB > the 126 MB L2), so nothing is served
+-> C ABI).  Every call has its own input tensors (12 distinct sets, ~1 GB > the 50 MB L2), so nothing is served
 from a warm cache between steps.
 
 Reported (one JSON line, rank 0):
@@ -18,9 +18,17 @@ Reported (one JSON line, rank 0):
                 (N*Lq*M*L*P per call), counted once per forward+backward pair.
   e2e        -- same metric with HOST (pinned) inputs and results: H2D of value/loc/attn/grad_out and D2H of
                 out/grad_value/grad_loc/grad_attn inside the timed region.
-  roofline   -- dominant kernel (encoder-shaped backward: zero-fill + msda_bwd_tiled) against the measured HBM peak.
+  roofline   -- dominant kernel (encoder-shaped backward: zero-fill + msda_bwd_tiled) against the HBM peak.
+  device     -- name and power limit of the GPU the numbers were measured on.
   cpu_baseline -- the reference's ms_deform_attn_core_pytorch CPU path (its own file, staged in oracle/_ref; the
                   torch port pinned to it when no staged copy exists) on this box's host cores.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller -- out, grad_value,
+grad_loc, grad_attn of each of the 12 calls -- as DIR/<call>_<array>.npy (float32): arrays of up to 2^16 elements whole,
+larger ones as a fixed seeded sample of 2^16 elements (DIR/<call>_<array>_index.npy holds their flat indices, stored as
+float64, exact below 2^53).  With the flag, the last timed step keeps its results alive until the dump instead of
+freeing them call by call.  The inputs
+depend only on the arguments (seeded), so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -65,6 +73,8 @@ def parse_args():
                     help="skip timing the reference's own layer classes on its own CUDA kernels (frames.reference_stack)")
     ap.add_argument("--frames-steps", type=int, default=5)
     ap.add_argument("--cpu-budget-s", type=float, default=25.0, help="target CPU seconds for the cpu_baseline sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (out / grad_value / grad_loc / grad_attn of every call) as .npy")
     return ap.parse_args()
 
 
@@ -75,27 +85,48 @@ def dist_env():
     return world, rank, local
 
 
-def ncu_traffic(tag, key):
-    """DRAM bytes per launch from the committed ncu --set full capture (tools/ncu_traffic.py), or None."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(p) as fh:
-            return int(json.load(fh)[tag][key]["dram_bytes"])
-    except (OSError, KeyError, ValueError):
-        return None
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as fh:
             d = json.load(fh)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured peak)"
+
+
+def device_identity(index):
+    """Name and power limit of the GPU the numbers are measured on (read-only nvidia-smi query)."""
+    res = {"name": torch.cuda.get_device_name(index), "sms": torch.cuda.get_device_properties(index).multi_processor_count}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", str(index)], capture_output=True, text=True, timeout=30)
+        f = [x.strip() for x in q.stdout.strip().split(",")]
+        res["power_limit_w"] = float(f[0])
+        res["sm_max_mhz"] = float(f[1])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        res["power_limit_w"] = None
+    return res
+
+
+def dump_outputs(dirname, calls, results):
+    """The last timed step's results as float32 .npy files; arrays above 2^16 elements as a fixed seeded sample."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    cap = 1 << 16
+    for i, (c, res) in enumerate(zip(calls, results)):
+        for name, t in zip(("out", "grad_value", "grad_loc", "grad_attn"), res):
+            flat = t.detach().reshape(-1)
+            stem = os.path.join(dirname, f"{c['kind']}{i % N_ENC}_{name}")
+            if flat.numel() > cap:
+                g = torch.Generator().manual_seed(i * 4 + len(name))
+                idx = torch.randperm(flat.numel(), generator=g)[:cap].sort().values
+                np.save(stem + "_index.npy", idx.numpy().astype(np.float64))
+                flat = flat[idx.to(flat.device)]
+            np.save(stem + ".npy", flat.float().cpu().numpy())
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -195,7 +226,7 @@ def run_b200(args):
         return (c["value"], c["spatial_shapes"], c["level_start_index"], c["sampling_locations"],
                 c["attention_weights"])
 
-    def step(ev=None):
+    def step(ev=None, keep=None):
         for i, c in enumerate(calls):
             a = op_args(c)
             if ev is not None:
@@ -206,6 +237,8 @@ def run_b200(args):
             grads = MSDA.ms_deform_attn_backward(*a, c["grad_output"], 64)
             if ev is not None:
                 ev[i][2].record()
+            if keep is not None:
+                keep.append((out, *grads))
         return out, grads
 
     def barrier():
@@ -228,13 +261,17 @@ def run_b200(args):
         time.sleep(0.25)
     barrier()
     launches0 = lib.msda_launch_count()
+    last = [] if args.dump_outputs else None
     t0.record()
     for k in range(K):
-        step(evs[k])
+        step(evs[k], keep=last if k == K - 1 else None)
     t1.record()
     barrier()
     launches = lib.msda_launch_count() - launches0
     total_ms = t0.elapsed_time(t1)
+    if last is not None and rank == 0:
+        dump_outputs(args.dump_outputs, calls, last)
+    del last
     clocks = sampler.stop() if rank == 0 else None
     if world > 1:
         import torch.distributed as dist
@@ -257,15 +294,6 @@ def run_b200(args):
     roofline = {"bound": "hbm", "kernel": "encoder-shaped backward: grad_value zero-fill (msda_zero_fill, PDL primary) + msda_bwd_tiled",
                 "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4),
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": b_bwd,
-                "traffic": ncu_traffic(f"{args.config}_enc_{'f32' if args.dtype == 'fp32' else 'bf16'}", "bwd"),
-                "traffic_note": "msda_bwd_tiled only (the 45.7 MB grad_value zero-fill is a separate launch); profiles/ncu_traffic.json",
-                "binding_ceiling": "backward: each SM's path into the crossbar carries ~25 B/clk of red.global payload (21.8 with all "
-                                   "148 SMs active; scales with the SM count, independent of the hot-set size -> it is not the L2 "
-                                   "atomic units; profiles/r02b_ubench_smem_rmw_and_egress.txt); the op must add 4 x 128 B per tap "
-                                   "(2.5 GB per call) -> 393 us + gathers.  Combining rows inside the SM removes egress one for one "
-                                   "but costs 4 shared-memory wavefronts per row on the LSU data pipe the gathers already keep > 50 % "
-                                   "busy (slab kernels: -43 % red sectors, +36 % time; profiles/r02c_slab_kernels_ncu.md).  forward: "
-                                   "LSU data pipe 66-72 % busy moving 2.93 GB of rows per call (>= 155 k wavefronts per SM)",
                 "enc_fwd": {"achieved": round(b_fwd / (kern["enc_fwd_ms"] * 1e-3) / 1e9, 1),
                             "frac": round(b_fwd / (kern["enc_fwd_ms"] * 1e-3) / 1e9 / peak, 4),
                             "algorithmic_bytes_per_launch": b_fwd}}
@@ -311,7 +339,7 @@ def run_b200(args):
                                "enc_bwd": round(cfg.samples("enc") / kern["enc_bwd_ms"] / 1e6, 2),
                                "dec_fwd": round(cfg.samples("dec") / kern["dec_fwd_ms"] / 1e6, 2),
                                "dec_bwd": round(cfg.samples("dec") / kern["dec_bwd_ms"] / 1e6, 2)},
-            "roofline": roofline, "e2e": e2e, "frames": frames, "gpu_launches": int(launches), "clocks": clocks,
+            "device": device_identity(local), "roofline": roofline, "e2e": e2e, "frames": frames, "gpu_launches": int(launches), "clocks": clocks,
             "cpu_baseline": cpu_base, "reference_cuda": ref_cuda, "configs": other_cfgs,
         }
         print(json.dumps(line), flush=True)
@@ -321,7 +349,7 @@ def run_b200(args):
 
 
 def _time_call(fn, iters=10, warm=3):
-    """Median CUDA-event time of fn() over `iters` runs, with a 256 MB write between runs to flush the 126 MB L2."""
+    """Median CUDA-event time of fn() over `iters` runs, with a 256 MB write between runs to flush the 50 MB L2."""
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     xs = []
     for i in range(warm + iters):
@@ -338,7 +366,7 @@ def _time_call(fn, iters=10, warm=3):
 
 def reference_cuda_leg(calls, op_args, kern):
     """The REAL bar (BASELINE.md 2b): the reference's own CUDA kernels -- ms_deform_im2col_cuda.cuh compiled unmodified
-    for sm_100a into oracle/_ref (oracle/build_refcuda.sh) -- timed on the same tensors of the same B200, OUTSIDE the
+    for sm_90a into oracle/_ref (oracle/build_refcuda.sh) -- timed on the same tensors of the same GPU, OUTSIDE the
     timed region of this bench.  oracle/ is used here only as a measured baseline, like cpu_baseline."""
     try:
         from oracle import refcuda
@@ -506,7 +534,7 @@ def build_reference_stack(cfg, tr_mod, num_layers=6, d_ffn=2048):
 def reference_stack_leg(cfg, device, steps, lib, inputs, ours):
     """The anchor for frames/s: the SAME step (6 + 6 layers fwd + bwd, same synthetic features, same loss) run by the
     REFERENCE's GPU stack -- its own Python classes (``DeformableTransformerEncoderLayer`` / ``DecoderLayer`` /
-    ``MSDeformAttn`` / ``MSDeformAttnFunction`` of deformable_transformer.py and ops/, unmodified files staged in tests/_ref)
+    ``MSDeformAttn`` / ``MSDeformAttnFunction`` of deformable_transformer.py and ops/, unmodified files staged by tests/stage_reference.py where a reference checkout exists)
     on its own CUDA kernels (ms_deform_im2col_cuda.cuh compiled unmodified into oracle/_ref/libmsda_refcuda.so).  None of
     this repo's kernels is on that path (checked with the library's launch counter).  Baseline leg only, outside every
     timed region of this repo's numbers, like `reference_cuda`."""
@@ -514,7 +542,7 @@ def reference_stack_leg(cfg, device, steps, lib, inputs, ours):
         from oracle import refcuda
         from tests import stage_reference
         if not stage_reference.staged():
-            return {"unavailable": "tests/_ref not staged (needs /root/reference at build time)"}
+            return {"unavailable": "reference files not staged (needs /root/reference at build time)"}
         if not refcuda.available():
             return {"unavailable": "oracle/_ref/libmsda_refcuda.so not built (needs /root/reference at build time)"}
         import warnings
@@ -549,7 +577,7 @@ def reference_stack_leg(cfg, device, steps, lib, inputs, ours):
                         "msda_b200_launches_per_step": int((lib.msda_launch_count() - l0) / steps)}
 
             res = {"what": "the reference's own layer classes (deformable_transformer.py:321-416, ops/modules, ops/functions; "
-                           "unmodified files, tests/_ref) on the reference's own CUDA kernels (oracle/_ref), eager PyTorch as "
+                           "unmodified files staged from a reference checkout) on the reference's own CUDA kernels (oracle/_ref), eager PyTorch as "
                            "the reference runs them; same step, features and loss as the legs above; single GPU"}
             old = torch.backends.cuda.matmul.allow_tf32
             try:
@@ -697,8 +725,7 @@ def setup_e2e(MSDA, calls, op_args, world, smp_step, steps, device, barrier):
                 "reps_ms_per_step": [round(x, 3) for x in reps],
                 "policy": f"median of {len(reps)} repetitions of {steps} timed steps each, spread over the run (after the "
                           "device-resident timing, after the frames leg, after the baseline legs): the host side of a shared "
-                          "box is bursty -- one run in eight measured a 3x slower PCIe leg on an otherwise normal box "
-                          "(profiles/r02zy_zero_fill_ab.txt)",
+                          "machine is bursty",
                 "api": "MultiScaleDeformableAttention.ms_deform_attn_forward/backward on pinned-host inputs; "
                        "H2D / kernels / D2H on three streams", "host_numa": numa}
 
@@ -729,7 +756,7 @@ def step_config(cfg, world):
             "heads": cfg.heads, "head_dim": cfg.head_dim, "points": cfg.points,
             "dec_queries": cfg.dec_queries, "calls_per_step": f"{N_ENC} enc + {N_DEC} dec, fwd+bwd",
             "samples_per_step_per_gpu": samples_per_step(cfg), "parallelism": f"dp{world} (frames sharded, no exchange)",
-            "l2_policy": "12 distinct input sets per step (~1 GB) > 126 MB L2"}
+            "l2_policy": "12 distinct input sets per step (~1 GB) > 50 MB L2"}
 
 
 def cpu_call(port, c):

@@ -1,5 +1,6 @@
 /*
- * msda_b200.h -- C ABI of the B200-native multi-scale deformable attention library (libmsda_b200.so).
+ * msda_b200.h -- C ABI of the sm_90a (H100) multi-scale deformable attention library (libmsda_b200.so; the name is
+ * historical).
  *
  * This is the drop-in boundary for the reference's native module `MultiScaleDeformableAttention`
  * (projects/UNINEXT/uninext/models/deformable_detr/ops/src/vision.cpp:13-16), whose two functions
@@ -11,7 +12,7 @@
  *
  * Conventions
  *   - every pointer is a DEVICE pointer on the current CUDA device, dense row-major.  16-byte aligned tensors (what
- *     any allocator returns) take the tiled / slab sm_100a kernels; a merely element-aligned pointer (a contiguous view
+ *     any allocator returns) take the tiled / slab sm_90a kernels; a merely element-aligned pointer (a contiguous view
  *     with a storage offset, which the reference accepts too) is served by the generic kernels:
  *       value              [N, S, M, D]          (reference: ms_deform_attn_cuda.cu:40-43)
  *       spatial_shapes     [L, 2] int64 (H_l,W_l)  -- read on the device, no host sync (cu:67)
@@ -43,16 +44,16 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 2   /* 2: round-2 entry points (knobs, CondInst head, geometry, W-stationary GEMM) */
+#define MSDA_ABI_VERSION 3   /* 3: sm_90 build; the GEMM timeline diagnostic is gone */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
-#define MSDA_E_NODEVICE (-3)   /* no sm_100 device is current                                          */
+#define MSDA_E_NODEVICE (-3)   /* no usable CUDA device is current                                     */
 
 int msda_abi_version(void);
 const char *msda_strerror(int code);
 
-/* Which kernel family a (dtype, D, L, P) problem is routed to: 1 = tiled sm_100a fast path, 0 = generic.
+/* Which kernel family a (dtype, D, L, P) problem is routed to: 1 = tiled sm_90a fast path, 0 = generic.
  * dtype_bytes: 2 (bf16), 4 (fp32), 8 (fp64). Used by the tests to prove the fast path is the one exercised. */
 int msda_uses_fast_path(int dtype_bytes, int D, int L, int P);
 
@@ -64,7 +65,8 @@ uint64_t msda_launch_count(void);
  * them to run every kernel family on small shapes, the tools to sweep them.  Returns the previous value, or
  * MSDA_E_BADARG for an unknown knob.  value == MSDA_KNOB_QUERY reads without writing.
  *   MSDA_KNOB_SLAB          1 = slab-ordered kernels (msda_slab.cuh) whenever D == 32 and L*P <= 16; 2 = tiled forward +
- *                           backward with tensor-memory accumulators for the coarse levels (msda_tmem.cuh); -1 (auto) and
+ *                           backward with the coarse levels accumulated by dedicated consumer warps in a shared-memory
+ *                           window (msda_tmem.cuh); -1 (auto) and
  *                           0 = tiled kernels
  *   MSDA_KNOB_BWD_WIN_ROWS  shared-memory window of the slab backward in rows of 128 B (-1 = all that fits)
  *   MSDA_KNOB_BWD_LIST_CAP  entries per row-class list of the slab backward (even, >= 8)
@@ -78,13 +80,12 @@ uint64_t msda_launch_count(void);
  *   MSDA_KNOB_ZERO_FILL             how msda_backward_* zero-fills grad_value (results identical): 0 = cudaMemsetAsync,
  *                                   1 = msda_zero_fill kernel (16-byte stores, one wave), 2 = the same kernel launched as the
  *                                   programmatic-dependent-launch primary of the tiled backward kernel, whose prologue then
- *                                   overlaps the fill (not while the stream is being captured into a CUDA graph).  Default 2
- *                                   (cfg2 on B200: step 4.186 -> 4.156 ms, decoder-shaped backward 26.7 -> 23.6 us). */
+ *                                   overlaps the fill (not while the stream is being captured into a CUDA graph).  Default 2. */
 #define MSDA_KNOB_SLAB          0
 #define MSDA_KNOB_BWD_WIN_ROWS  1
 #define MSDA_KNOB_BWD_LIST_CAP  2
 #define MSDA_KNOB_FWD_SLAB_CTAS 3
-#define MSDA_KNOB_F32_VEC8_FWD  4   /* fp32 tiled forward: 8 channels per lane (LDG.256), D in {32, 64}; 0 / 1        */
+#define MSDA_KNOB_F32_VEC8_FWD  4   /* fp32 tiled forward: 8 channels per lane (2 x 16 B), D in {32, 64}; 0 / 1      */
 #define MSDA_KNOB_F32_VEC8_BWD  5   /* fp32 tiled backward: same lane shape; 0 / 1                                     */
 #define MSDA_KNOB_BF16_FINE_ROWS 6  /* bf16 backward: levels with H*W >= this accumulate grad_value in bf16; 0 = off */
 #define MSDA_KNOB_BF16_PACKED_FWD 7 /* bf16 forward: corners of a tap blended in packed bf16 (HFMA2); 0 / 1            */
@@ -199,23 +200,18 @@ int msda_aligned_bilinear_forward_f32(const float *in, int64_t planes, int h, in
 int msda_aligned_bilinear_backward_f32(const float *grad_out, int64_t planes, int h, int w, int factor, float *grad_in,
                                        void *stream);
 
-/* ---- tcgen05 GEMM for the Linears that bracket the op:  C[M,N] = A[M,K] . W[N,K]^T + bias[N]  (fp32 storage, TF32 MMA
- * with fp32 accumulation in tensor memory; TMA-fed).  K % 32 == 0, N % 32 == 0 (N % 64 == 0 above 256), N <= 512.
+/* ---- TF32 GEMM for the Linears that bracket the op:  C[M,N] = A[M,K] . W[N,K]^T + bias[N]  (fp32 storage, sm_90 wgmma TF32
+ * MMA with fp32 accumulation; TMA-fed).  K % 32 == 0, N % 32 == 0 (N % 64 == 0 above 256), N <= 512.
  * Replaces torch.nn.functional.linear for value_proj / output_proj / the concatenated sampling projection
  * (ops/modules/ms_deform_attn.py:95,99-100,115) when TF32 GEMMs are allowed. bias may be NULL. */
 int msda_linear_tf32(const float *A, const float *W, const float *bias, int64_t M, int N, int K, float *C, void *stream);
-/* W-stationary variant with a fused tail, for K <= 256 and N <= 256 (N % 64 == 0; msda_linear_tf32_ws_ok tells):
+/* The same GEMM with a fused tail, for N <= 256 (N % 64 == 0; msda_linear_tf32_ws_ok tells):
  *   C = A . W^T + bias;  rows with row_mask[m] != 0 are written as zeros (the `masked_fill(input_padding_mask)` that follows
  *   value_proj, ops/modules/ms_deform_attn.py:96-97);  relu != 0 applies max(., 0) (FFN linear1).  bias / row_mask may be NULL.
- *   msda_linear_tf32 itself routes eligible shapes to this kernel.  Two implementations: for K <= 256 a 2-CTA MMA kernel
- *   (tcgen05.mma.cta_group::2, M = 256 per CTA pair, TMA-store epilogue), otherwise / with MSDA_GEMM_WS2=0 the 1-CTA kernel
- *   with multicast A.  A, W, C (and bias) must be 16-byte aligned. */
+ *   A, W, C (and bias) must be 16-byte aligned. */
 int msda_linear_tf32_ex(const float *A, const float *W, const float *bias, const uint8_t *row_mask, int64_t M, int N, int K,
                         int relu, float *C, void *stream);
 int msda_linear_tf32_ws_ok(int N, int K);
-/* Diagnostic: phase timeline of the last 2-CTA W-stationary GEMM launched with MSDA_GEMM_WS_DBG=1 (160 CTAs x 24 slots of
- * SM-clock stamps; layout in msda_gemm_sm100.cu).  Copies min(n_words, 3840) words to `out` (host). */
-int msda_debug_gemm_timeline(unsigned long long *out, int n_words);
 
 #ifdef __cplusplus
 }

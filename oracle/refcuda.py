@@ -1,8 +1,8 @@
 """TEST / BENCH INFRASTRUCTURE ONLY -- ctypes face of oracle/_ref/libmsda_refcuda.so, i.e. the REFERENCE's own CUDA
-kernels (ms_deform_im2col_cuda.cuh, compiled unmodified for sm_100a by oracle/build_refcuda.sh).
+kernels (ms_deform_im2col_cuda.cuh, compiled unmodified for sm_90a by oracle/build_refcuda.sh).
 
 Used by tests/ (parity against the reference op itself on identical tensors) and by tools/opbench.py (the reference
-kernels timed on the same B200). Never imported by the product package.
+kernels timed on the same GPU). Never imported by the product package.
 """
 import ctypes
 import os

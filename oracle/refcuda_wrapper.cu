@@ -1,7 +1,7 @@
 // TEST / BENCH INFRASTRUCTURE ONLY -- exposes the REFERENCE's own CUDA kernels (compiled unmodified from where they
 // lie under /root/reference, see oracle/build_refcuda.sh) through a C ABI, so that on the GPU box
-//   * parity tests can compare the sm_100a kernels against the reference op itself on identical tensors, and
-//   * bench tools can time the reference kernels (K1 forward, K2 backward) on the same B200.
+//   * parity tests can compare the sm_90a kernels against the reference op itself on identical tensors, and
+//   * bench tools can time the reference kernels (K1 forward, K2 backward) on the same GPU.
 // Only the two templated launchers of ms_deform_im2col_cuda.cuh are used (cuh:923-954, cuh:956-1327); the ATen host
 // wrapper ms_deform_attn_cuda.cu is not (it needs torch 1.x's Tensor::type()).  No reference source is copied here.
 #include <cstdint>

@@ -1,11 +1,10 @@
 """TEST INFRASTRUCTURE ONLY -- the reference's OWN CPU path, ``ms_deform_attn_core_pytorch``
 (``ops/functions/ms_deform_attn_func.py:43-63``), loaded from the reference file itself.
 
-Same status as ``oracle/_ref/libmsda_refcuda.so`` (the reference's CUDA kernels compiled where they lie): in the build
-container ``stage()`` (called by ``__graft_entry__.build()``) copies the one reference file byte for byte into the
-git-ignored ``oracle/_ref/``; it travels to the GPU box with the gpurun snapshot and never enters history.  Users:
-``bench.py``'s ``cpu_baseline`` leg and ``--impl reference`` arm (which then report ``kind: "reference"`` instead of
-``"port"``) and ``tests/``.  Nothing under ``uninext_b200/`` imports this module.
+Where a reference checkout exists, ``stage()`` (run by hand, e.g. by tests/golden/make_reference_golden.py) copies the
+one reference file byte for byte into the git-ignored ``oracle/_ref/``; it never enters history.  Users: the golden
+generator, and ``bench.py``'s ``cpu_baseline`` leg and ``--impl reference`` arm, which report ``kind: "reference"``
+when a staged copy exists and otherwise time the port (``kind: "port"``) that the stored reference results pin.  Nothing under ``uninext_b200/`` imports this module.
 
 The file imports the compiled extension ``MultiScaleDeformableAttention`` at module level (``func.py:18``) although the
 CPU function never touches it; it is loaded here against an EMPTY stand-in module so that the reference arm loads none
@@ -21,14 +20,15 @@ import types
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _REL = "projects/UNINEXT/uninext/models/deformable_detr/ops/functions/ms_deform_attn_func.py"
-SOURCE = os.path.join("/root/reference", _REL)
+REFERENCE = os.environ.get("UNINEXT_REFERENCE", "/root/reference")      # a checkout of the reference repository
+SOURCE = os.path.join(REFERENCE, _REL)
 STAGED = os.path.join(_HERE, "_ref", "ms_deform_attn_func.py")
 
 _cached = None
 
 
 def stage() -> bool:
-    """Copy the reference file into oracle/_ref/ (build container only). True when a staged copy exists afterwards."""
+    """Copy the reference file into oracle/_ref/ (where a reference checkout exists). True when a staged copy exists afterwards."""
     if os.path.isfile(SOURCE):
         os.makedirs(os.path.dirname(STAGED), exist_ok=True)
         if not os.path.exists(STAGED) or os.path.getmtime(STAGED) < os.path.getmtime(SOURCE):

@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and shared fixtures.
 
 `-m "not gpu"` runs here on CPU (oracle vs golden vectors, host logic, C-ABI symbol export, gloo world_size-2);
-`-m gpu` runs on a B200 and calls the CUDA path through the C-ABI.
+`-m gpu` runs on an H100 and calls the CUDA path through the C-ABI.
 """
 import glob
 import os
@@ -18,7 +18,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_sessionstart(session):
@@ -32,11 +32,6 @@ def pytest_sessionstart(session):
         _o.build()
     except Exception as exc:                       # no nvcc / gcc here: the tests that need the libraries will say so
         print(f"[conftest] native build skipped: {exc}")
-    try:                                           # reference Python files for the "reference classes on the drop-in" tests
-        from tests import stage_reference          # (copies only where /root/reference exists; git-ignored tests/_ref)
-        stage_reference.stage()
-    except Exception as exc:
-        print(f"[conftest] reference staging skipped: {exc}")
 
 
 def golden_names():

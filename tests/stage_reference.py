@@ -1,14 +1,13 @@
 #!/usr/bin/env python
-"""TEST INFRASTRUCTURE -- stage the reference's own Python files of the hot path into the git-ignored ``tests/_ref/``
-so that ``-m gpu`` tests can run the REFERENCE classes (``MSDeformAttnFunction``, ``MSDeformAttn``,
-``DeformableTransformerEncoderLayer`` / ``DecoderLayer`` / ``DeformableReidHead``) unchanged on top of the sm_100a
-drop-in, on the GPU box where ``/root/reference`` does not exist.
+"""TEST INFRASTRUCTURE -- stage the reference's own Python files of the hot path into the git-ignored
+``oracle/_ref/py/`` where a reference checkout exists, so that tests/golden/make_reference_golden.py can record the
+results of the REFERENCE classes and functions, and tools/condinst_bench.py / bench.py's reference_stack leg can time
+them.  The tests themselves never read these copies: they compare with tests/golden/reference/.  build() does not stage.
 
-    python tests/stage_reference.py            # copies; no-op (exit 0) when /root/reference is absent
+    python tests/stage_reference.py            # copies; no-op (exit 0) when the reference checkout is absent
 
-Same status as ``oracle/_ref`` (the reference's CUDA kernels compiled where they lie): the copies are byte-identical
-to the reference, are never committed (``tests/_ref/`` is in .gitignore, not in .gpurunignore, so it travels with the
-gpurun snapshot), and nothing under ``uninext_b200/`` imports them. What is copied, verbatim:
+The copies are byte-identical to the reference, are never committed (``oracle/_ref/`` is in .gitignore), and nothing
+under ``uninext_b200/`` imports them. What is copied, verbatim:
 
     ops/functions/{__init__,ms_deform_attn_func}.py       (a1/a2: the autograd boundary)
     ops/modules/{__init__,ms_deform_attn}.py              (a9)
@@ -26,9 +25,12 @@ import shutil
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-DEST = os.path.join(HERE, "_ref")
+DEST = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "py")
 PKG = os.path.join(DEST, "uninext_ref")
-SRC = "/root/reference/projects/UNINEXT/uninext/models/deformable_detr"
+sys.path.insert(0, os.path.dirname(HERE))
+from oracle.refpy import REFERENCE  # noqa: E402
+
+SRC = os.path.join(REFERENCE, "projects/UNINEXT/uninext/models/deformable_detr")
 
 COPIES = [
     "ops/functions/__init__.py",
@@ -80,7 +82,7 @@ def staged() -> bool:
 
 
 def stage(force: bool = False) -> bool:
-    """Returns True when tests/_ref is usable afterwards."""
+    """Returns True when the staged copies are usable afterwards."""
     if not os.path.isdir(SRC):
         return staged()
     if staged() and not force:
@@ -130,4 +132,4 @@ def import_ddetrs():
 
 if __name__ == "__main__":
     ok = stage(force="--force" in sys.argv)
-    print(f"tests/_ref {'ready' if ok else 'NOT staged (no /root/reference here)'}")
+    print(f"{DEST} {'ready' if ok else 'NOT staged (no reference checkout here)'}")

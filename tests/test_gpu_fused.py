@@ -135,7 +135,7 @@ def test_linear_relu_and_split_k_weight_grad():
 @pytest.mark.parametrize("m,n,k", [(128, 256, 256), (1, 32, 32), (300, 256, 256), (1000, 384, 256), (44646, 256, 256),
                                    (44646, 384, 256), (513, 512, 64), (77, 32, 96), (200, 448, 128), (129, 64, 512)])
 def test_tcgen05_linear_matches_fp64_within_tf32(m, n, k):
-    """Hand-written tcgen05 GEMM (TMA multicast, TMEM accumulators): TF32 operands (10-bit mantissa), fp32 accumulate."""
+    """Hand-written TF32 GEMM (sm_90a wgmma, TMA-fed): TF32 operands (10-bit mantissa), fp32 accumulate."""
     from uninext_b200.functions.fused import tcgen05_linear, tcgen05_linear_ok
     torch.manual_seed(6)
     a = torch.randn(m, k, device=DEV)

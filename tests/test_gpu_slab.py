@@ -1,14 +1,12 @@
 """GPU tests (-m gpu) of the kernel families selected by `msda_set_knob`: the slab-ordered kernels
-(uninext_b200/csrc/msda_slab.cuh: LDG.256 forward, backward with a shared-memory window for the coarse levels of
-grad_value), the backward with tensor-memory accumulators (msda_tmem.cuh), the 32-byte lane shape of the fp32 tiled
+(uninext_b200/csrc/msda_slab.cuh: 32-byte-lane forward, backward with a shared-memory window for the coarse levels of
+grad_value), the backward with dedicated consumer warps (msda_tmem.cuh), the 32-byte lane shape of the fp32 tiled
 kernels and the mixed bf16 / fp32 accumulation of the bf16 backward.  The knobs force them onto small and ragged problems
 so that every branch -- window level sets, list overflow falling back to red.global, partial tiles, CTAs spanning
 several slabs -- is compared with the fp64 oracle and with the default tiled kernels.
 
-The slab kernels are an OPT-IN family (MSDA_KNOB_SLAB=1): measured on B200 they cut L2 traffic (forward: -48 % L2 sectors,
-L1 hit rate 34 % -> 65 %; backward: -43 % red sectors) but not run time, because the SM's load/store data pipe, not
-L2 or the crossbar, is the wall for both (profiles/r02c_slab_kernels_ncu.md).  They stay tested so the evidence can be
-reproduced."""
+The slab kernels are an OPT-IN family (MSDA_KNOB_SLAB=1): they cut L2 traffic but are not the default kernels.  They
+stay tested so that they can be measured again."""
 import numpy as np
 import pytest
 import torch
@@ -147,7 +145,7 @@ def test_slab_and_tiled_kernels_agree_at_cfg2(knobs):
 
 @pytest.mark.parametrize("kind", ["enc", "dec"])
 def test_f32_vec8_lane_shape_vs_oracle(knobs, kind):
-    """fp32 tiled kernels with 4 lanes x 32 B per row (LDG.256) instead of 8 lanes x 16 B."""
+    """fp32 tiled kernels with 4 lanes x 32 B per row instead of 8 lanes x 16 B."""
     knobs.msda_set_knob(_cabi.KNOB_F32_VEC8_FWD, 1)
     knobs.msda_set_knob(_cabi.KNOB_F32_VEC8_BWD, 1)
     _check(make_inputs(CONFIGS["cfg1"], kind, DEV, seed=29, wild_fraction=0.1), 1e-4)
@@ -170,7 +168,7 @@ def test_f32_vec8_ragged_vs_oracle(knobs, D):
 
 # cfg1 levels have 1600 / 400 / 100 / 25 rows: threshold 500 = the finest level accumulates in bf16, 5000 = none (all fp32,
 # but through the mixed code path).  Lower thresholds put the small, heavily-hit levels into bf16 too and leave the 1e-2
-# tolerance (measured 3-7 % on the coarsest level, profiles/r02g_bf16_mixed_accumulation.txt): not a supported setting.
+# tolerance: not a supported setting.
 @pytest.mark.parametrize("fine_rows", [500, 5000])
 def test_bf16_backward_mixed_accumulation_vs_oracle(knobs, fine_rows):
     """bf16 backward with the big levels' grad_value accumulated directly in the bf16 result (packed reds) and the small
@@ -183,7 +181,7 @@ def test_bf16_backward_mixed_accumulation_vs_oracle(knobs, fine_rows):
     assert knobs.msda_launch_count() - before == 4          # forward, zero coarse scratch rows, backward, round coarse rows
 
 
-# ---- tensor-memory backward (msda_tmem.cuh, MSDA_KNOB_SLAB = 2): coarse levels of grad_value accumulated in TMEM columns ----
+# ---- consumer-warp backward (msda_tmem.cuh, MSDA_KNOB_SLAB = 2): coarse levels of grad_value accumulated in shared memory ----
 @pytest.mark.parametrize("kind", ["enc", "dec"])
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 1e-4), (torch.bfloat16, 1e-2)])
 @pytest.mark.parametrize("list_cap", [48, 8])                  # 8: producer lists overflow -> red.global fallback

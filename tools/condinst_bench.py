@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """CondInst dynamic mask head: this repo's fused kernels vs the REFERENCE function (staged uninext/models/ddetrs.py:
-repeat + three grouped convolutions + aligned_bilinear) on the same B200, forward and forward+backward.
-    python tools/condinst_bench.py          (needs tests/_ref staged: python tests/stage_reference.py)"""
+repeat + three grouped convolutions + aligned_bilinear) on the same GPU, forward and forward+backward.
+    python tools/condinst_bench.py          (needs the reference files staged: python tests/stage_reference.py)"""
 import json
 import os
 import sys

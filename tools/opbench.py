@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmark of single MSDeformAttn calls (CUDA events, L2 flushed between iterations).
     python tools/opbench.py --config cfg2 --kind enc --dtype fp32 --iters 20
-Also the short command that ncu wraps (see tools/gpu_profile.sh)."""
+Also a short command to run under a profiler."""
 import argparse
 import json
 import os

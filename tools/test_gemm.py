@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Bring-up check for msda_linear_tf32 (tcgen05 GEMM): compare with torch (TF32 tolerance), then time it vs cuBLAS."""
+"""Bring-up check for msda_linear_tf32 (wgmma TF32 GEMM): compare with torch (TF32 tolerance), then time it vs cuBLAS."""
 import os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -29,7 +29,7 @@ if not ok:
 torch.backends.cuda.matmul.allow_tf32 = True
 for (m, n, k) in [(44646, 256, 256), (44646, 384, 256)]:
     a = torch.randn(m, k, device="cuda"); w = torch.randn(n, k, device="cuda") * 0.1; b = torch.randn(n, device="cuda")
-    for name, fn in (("tcgen05", lambda: linear_tf32(a, w, b)), ("cublas-tf32", lambda: torch.addmm(b, a, w.t()))):
+    for name, fn in (("wgmma-tf32", lambda: linear_tf32(a, w, b)), ("cublas-tf32", lambda: torch.addmm(b, a, w.t()))):
         for _ in range(5): fn()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -1,6 +1,6 @@
 // Micro-benchmark: TMA bulk reduction (cp.reduce.async.bulk ... add.f32) of 128-byte rows from shared memory into random
 // rows of an L2-resident fp32 table, vs the LSU path (red.global.add.v4.f32) measured by ubench_gather.cu.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench_bulkred tools/ubench_bulkred.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench_bulkred tools/ubench_bulkred.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

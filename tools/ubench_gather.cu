@@ -1,5 +1,5 @@
 // Micro-benchmark: what does one SM sustain for "4 rows x 128 B per LDG.128" gathers (the op's access shape)?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench_gather tools/ubench_gather.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench_gather tools/ubench_gather.cu
 // Prints cycles per LDG.128 warp-instruction per SM for several table sizes (L1-resident ... L2-resident), for
 // 8-lane x 16 B (fp32 rows) and 4-lane x 16 B (bf16 rows) and 32-lane x 4 B (reference-style scalar) shapes.
 #include <cstdio>

@@ -1,4 +1,4 @@
-"""uninext_b200 -- B200-native (sm_100a) multi-scale deformable attention: the hot path of UNINEXT's deformable
+"""uninext_b200 -- H100-native (sm_90a) multi-scale deformable attention (the package name is historical): the hot path of UNINEXT's deformable
 transformer, behind the reference's own operator boundary.
 
 Layout
@@ -16,7 +16,7 @@ __version__ = "0.1.0"
 
 def install_dropin() -> None:
     """Make ``import MultiScaleDeformableAttention`` (reference ops/functions/ms_deform_attn_func.py:18) resolve to
-    the sm_100a implementation."""
+    the sm_90a implementation."""
     from uninext_b200.dropin import MultiScaleDeformableAttention as _m
     _sys.modules["MultiScaleDeformableAttention"] = _m
 

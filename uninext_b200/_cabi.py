@@ -46,9 +46,8 @@ SIGNATURES = {
     "msda_condinst_backward_f32": (_i, [_vp] * 5 + [_i] * 7 + [_vp] * 4),
     "msda_aligned_bilinear_forward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
     "msda_aligned_bilinear_backward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
-    "msda_debug_gemm_timeline": (_i, [_vp, _i]),
 }
-ABI_VERSION = 2
+ABI_VERSION = 3
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL) = range(9)                                                      # include/msda_b200.h
 

@@ -1,9 +1,9 @@
-"""In-tree build of libmsda_b200.so (the C-ABI CUDA library) with nvcc for sm_100a.
+"""In-tree build of libmsda_b200.so (the C-ABI CUDA library) with nvcc for sm_90a (H100).
 
     python -m uninext_b200.build [--force] [--verbose]
 
-The library is a plain shared object (no torch / pybind dependency): nvcc cross-compiles it in seconds without a GPU,
-and it travels to the GPU box inside the repo snapshot (``uninext_b200/lib/`` is git-ignored, not gpurun-ignored).
+The library is a plain shared object (no torch / pybind dependency): nvcc cross-compiles it without a GPU.  It is built
+into ``uninext_b200/lib/`` (git-ignored), so a built tree can be copied to a GPU machine and run there as is.
 """
 from __future__ import annotations
 
@@ -19,11 +19,11 @@ LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmsda_b200.so")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
-SOURCES = ["msda_cabi.cu", "msda_gemm_sm100.cu"]
+SOURCES = ["msda_cabi.cu", "msda_gemm_sm90.cu"]
 HEADERS = ["msda_common.cuh", "msda_tiled.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--shared", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",

@@ -43,7 +43,7 @@ int num_sms() {
     const int dev = current_device();
     int v = sms[dev].load(std::memory_order_relaxed);
     if (v == 0) {
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         sms[dev].store(v, std::memory_order_relaxed);
     }
     return v;
@@ -68,7 +68,7 @@ struct Knobs {
         v[MSDA_KNOB_F32_VEC8_BWD].store(env_int("MSDA_F32_VEC8_BWD", 0));
         v[MSDA_KNOB_BF16_FINE_ROWS].store(env_int("MSDA_BF16_FINE_ROWS", 0));
         v[MSDA_KNOB_BF16_PACKED_FWD].store(env_int("MSDA_BF16_PACKED_FWD", 0));
-        v[MSDA_KNOB_ZERO_FILL].store(env_int("MSDA_ZERO_FILL", 2));   // measured: profiles/r02zy_zero_fill_ab.txt
+        v[MSDA_KNOB_ZERO_FILL].store(env_int("MSDA_ZERO_FILL", 2));
     }
 };
 Knobs &knobs() { static Knobs k; return k; }
@@ -131,11 +131,9 @@ int resident_ctas_cached(K kernel, std::atomic<int> (&cache)[kMaxDevices]) {
     return v;
 }
 
-// Slot order.  Measured on B200 (profiles/r01c_*_ncu.md, gpurun_out r01d sweep): the 8x8-pixel patch order lifts the
-// forward L1 sector hit rate from 39% to 75% and cuts L2 traffic 2.4x, but the kernels are bound by the LSU's
-// global-load issue rate (~7.5 cycles per 512-byte LDG.128 per SM), not by L1 misses, so run time does not move while
-// partially filled border patches cost 7-15% idle slots.  Linear order is therefore the default; MSDA_PATCHES=1
-// re-enables the patch order for experiments.
+// Slot order.  The 8x8-pixel patch order raises the forward's L1 hit rate and cuts L2 traffic, but the kernels are bound
+// by the LSU's global-load issue rate, not by L1 misses, while partially filled border patches leave slots idle.  Linear
+// order is therefore the default; MSDA_PATCHES=1 re-enables the patch order for experiments.
 int allow_patches() {
     static int v = -1;
     if (v < 0) { const char *e = getenv("MSDA_PATCHES"); v = (e && e[0] == '1') ? 1 : 0; }
@@ -156,8 +154,8 @@ bool use_split(unsigned npairs) {
     static int force = -2;
     if (force == -2) { const char *e = getenv("MSDA_SPLIT"); force = (e && (e[0] == '0' || e[0] == '1')) ? e[0] - '0' : -1; }
     if (force >= 0) return force == 1;
-    // measured (gpurun r01p): 4 800 pairs (cfg2 decoder call) fwd 18.4 -> 14.4 us, bwd 29.7 -> 27.6 us; neutral-to-worse
-    // from 14 400 pairs up, so only launches with fewer than ~56 pairs per SM are split
+    // splitting is meant for decoder-sized launches (cfg2: 4 800 pairs), whose few pairs cannot hide the row-load latency
+    // with other warps: launches with fewer than ~56 pairs per SM are split
     return npairs <= (unsigned)num_sms() * 56u;
 }
 
@@ -251,14 +249,13 @@ cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes,
 }
 
 // ---- slab-ordered kernels (msda_slab.cuh): D = 32 and L*P <= 16 (every UNINEXT call) ------------------------------
-// OPT-IN (MSDA_KNOB_SLAB = 1).  Measured at cfg2 (gpurun r02c, profiles/r02c_slab_kernels_ncu.md): forward 0.186 ms against
-// 0.175 ms tiled although L2 sectors halve and the L1 hit rate doubles; backward 0.654 ms against 0.480 ms although red
-// sectors drop 43 % -- the shared-memory traffic of the window (4 wavefronts per privatised row-add) lands on the same
-// LSU data pipe that the gathers already keep > 50 % busy.  MSDA_KNOB_SLAB = -1 (auto) therefore selects the tiled kernels.
+// OPT-IN (MSDA_KNOB_SLAB = 1).  They halve L2 sectors, but the shared-memory traffic of the window (4 wavefronts per
+// privatised row-add) lands on the same LSU data pipe that the gathers already keep busy, and they were slower than the
+// tiled kernels where they were first measured.  MSDA_KNOB_SLAB = -1 (auto) therefore selects the tiled kernels.
 
 bool use_slab(const Dims &d, unsigned npairs, const void *value, const void *out) {
     if (d.D != 32 || d.L * d.P > 16 || d.L > msda::kMaxLevels) return false;
-    if ((reinterpret_cast<uintptr_t>(value) & 31u) || (reinterpret_cast<uintptr_t>(out) & 15u)) return false;   // LDG.256 rows
+    if ((reinterpret_cast<uintptr_t>(value) & 31u) || (reinterpret_cast<uintptr_t>(out) & 15u)) return false;   // 32-byte row slices
     (void)npairs;
     return knob(MSDA_KNOB_SLAB) == 1;
 }
@@ -339,28 +336,38 @@ cudaError_t launch_bwd_mixed(const __nv_bfloat16 *go, const __nv_bfloat16 *value
     return cudaGetLastError();
 }
 
-// Backward with tensor-memory accumulators for the coarse levels (msda_tmem.cuh): MSDA_KNOB_SLAB = 2.
+// Backward with the coarse levels accumulated by dedicated consumer warps (msda_tmem.cuh): MSDA_KNOB_SLAB = 2.  The window
+// gets the device's opt-in shared memory minus the lists / g stash / tap slabs.
 template <typename T>
 cudaError_t launch_bwd_tmem(const T *grad_out, const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
                             const float *attn, const Dims &d, float *gv, float *gl, float *ga, cudaStream_t st) {
-    static std::atomic<int> ready[kMaxDevices], cap_c[kMaxDevices], epoch_c[kMaxDevices];
+    static std::atomic<int> win_rows[kMaxDevices], cap_c[kMaxDevices], epoch_c[kMaxDevices];
     const int dev = current_device();
     const int epoch = knobs().epoch.load(std::memory_order_acquire);
     auto kern = msda::msda_bwd_tmem<T, 16>;
-    int cap = cap_c[dev].load(std::memory_order_relaxed);
-    if (!ready[dev].load(std::memory_order_relaxed) || epoch_c[dev].load(std::memory_order_relaxed) != epoch) {
+    int cap = cap_c[dev].load(std::memory_order_relaxed), rows = win_rows[dev].load(std::memory_order_relaxed);
+    if (rows == 0 || epoch_c[dev].load(std::memory_order_relaxed) != epoch) {
         cap = knob(MSDA_KNOB_BWD_LIST_CAP) & ~1;
         if (cap < 8) cap = 8;
         if (cap > 128) cap = 128;
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msda::bwd_tmem_smem_bytes(cap));
+        int max_optin = 0;
+        cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        cudaFuncAttributes fa{};
+        cudaFuncGetAttributes(&fa, kern);
+        const long long fixed = (long long)msda::bwd_tmem_smem_bytes(cap, 0) + (long long)fa.sharedSizeBytes + 64;
+        rows = (int)((max_optin - fixed) / 128) & ~(msda::kTmCons - 1);
+        if (rows < 0) rows = 0;
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)msda::bwd_tmem_smem_bytes(cap, rows));
         if (e != cudaSuccess) return e;
         cap_c[dev].store(cap, std::memory_order_relaxed);
+        win_rows[dev].store(rows == 0 ? -1 : rows, std::memory_order_relaxed);
         epoch_c[dev].store(epoch, std::memory_order_relaxed);
-        ready[dev].store(1, std::memory_order_relaxed);
     }
+    if (rows < 0) rows = 0;
     const int sms = num_sms();
-    kern<<<sms, msda::kTmThreads, msda::bwd_tmem_smem_bytes(cap), st>>>(grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L,
-                                                                        d.Lq, d.P, sms, cap, gv, gl, ga);
+    kern<<<sms, msda::kTmThreads, msda::bwd_tmem_smem_bytes(cap, rows), st>>>(grad_out, value, shapes, lsi, loc, attn, d.N, d.S,
+                                                                              d.M, d.L, d.Lq, d.P, sms, cap, rows, gv, gl, ga);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
 }
@@ -374,7 +381,7 @@ cudaError_t fwd_fast(const T *value, const int64_t *shapes, const int64_t *lsi, 
     const int LP = d.L * d.P;
     if (use_slab(d, (unsigned)((long long)d.N * d.Lq * d.M), value, out))
         return launch_fwd_slab<T>(value, shapes, lsi, loc, attn, d, out, st);
-    if constexpr (sizeof(T) == 4) {           // fp32, 32-byte lanes (LDG.256): needs 32-byte aligned rows
+    if constexpr (sizeof(T) == 4) {           // fp32, 32-byte lanes: needs 32-byte aligned rows
         if (knob(MSDA_KNOB_F32_VEC8_FWD) == 1 && LP <= 16 && (d.D == 32 || d.D == 64) &&
             !(reinterpret_cast<uintptr_t>(value) & 31u))
             return d.D == 32 ? launch_fwd<T, 32, 16, 8>(value, shapes, lsi, loc, attn, d, out, st)

@@ -1,4 +1,4 @@
-// msda_common.cuh -- shared device helpers for the sm_100a multi-scale deformable attention kernels.
+// msda_common.cuh -- shared device helpers for the sm_90a multi-scale deformable attention kernels.
 //
 // Semantics follow the reference kernels in
 //   /root/reference/projects/UNINEXT/uninext/models/deformable_detr/ops/src/cuda/ms_deform_im2col_cuda.cuh ("cuh"):
@@ -88,14 +88,13 @@ template <> struct RowVec<float, 4> {
     }
 };
 
-// fp32, 8 channels per lane: one 32-byte access (sm_100 LDG.256 / STG.256 would need 32-byte alignment of the tensor, which
-// the router checks).  4 lanes cover a 128-byte row, 8 rows per warp instruction: 119 B/clk/SM from L1 against 80 for the
-// 16-byte shape (profiles/r02b_ubench_smem_rmw_and_egress.txt).
+// fp32, 8 channels per lane: two 16-byte loads (4 lanes cover a 128-byte row, 8 rows per warp instruction pair).  The
+// router still requires 32-byte aligned tensors for this shape.
 template <> struct RowVec<float, 8> {
     static constexpr int kElems = 8;
     __device__ static __forceinline__ void load(const float *p, float (&v)[8]) {
-        asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-            : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p));
+        const float4 a = __ldg(reinterpret_cast<const float4 *>(p)), b = __ldg(reinterpret_cast<const float4 *>(p) + 1);
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
     }
     __device__ static __forceinline__ void store(float *p, const float (&v)[8]) {
         reinterpret_cast<float4 *>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);

@@ -39,18 +39,16 @@ constexpr int kCiChunk = 16;                // instances whose parameters are st
 constexpr int kCiFwdGroups = 1;             // forward: groups of 4 pixels per thread (2: same time at 190 registers)
 constexpr int kCiFwdPpt = 4 * kCiFwdGroups, kCiBwdPpt = 2;      // pixels per thread
 
-// ---- packed fp32 pairs (FFMA2 = `fma.rn.f32x2`): the kernels keep two neighbouring pixels in the halves of a 64-bit register
-// pair.  A pair built from the same scalar twice compiles to FFMA2's scalar-broadcast operand, so a parameter costs one
-// 32-bit register read for two FMAs.  Measured issue cost per scheduler (tools/ubench_ffma.cu): FFMA with three registers
-// 1.5 cycles, FFMA2 with a broadcast multiplier 2.25 cycles per TWO FMAs -- the register file's read ports, not the fp32
-// lanes, set the rate -- and half the issue slots are left for the shared-memory reads of the parameters.
-struct f2 { unsigned long long v; };
-__device__ __forceinline__ f2 f2_make(float lo, float hi) { f2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi)); return r; }
+// ---- fp32 pairs: the kernels keep two neighbouring pixels in one pair of registers.  A pair built from the same scalar
+// twice costs one 32-bit shared-memory read for two FMAs.  sm_90 has no packed fp32 FMA, so a pair operation is two FFMAs
+// (each rounded once, exactly like the packed instruction would round each half).
+struct f2 { float lo, hi; };
+__device__ __forceinline__ f2 f2_make(float lo, float hi) { return f2{lo, hi}; }
 __device__ __forceinline__ f2 f2_bcast(float a) { return f2_make(a, a); }
-__device__ __forceinline__ float f2_lo(f2 a) { float lo, hi; asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v)); return lo; }
-__device__ __forceinline__ float f2_hi(f2 a) { float lo, hi; asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v)); return hi; }
-__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { f2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v)); return r; }
-__device__ __forceinline__ f2 f2_mul(f2 a, f2 b) { f2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
+__device__ __forceinline__ float f2_lo(f2 a) { return a.lo; }
+__device__ __forceinline__ float f2_hi(f2 a) { return a.hi; }
+__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { return f2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ f2 f2_mul(f2 a, f2 b) { return f2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
 __device__ __forceinline__ f2 f2_relu(f2 a) { return f2_make(fmaxf(f2_lo(a), 0.f), fmaxf(f2_hi(a), 0.f)); }
 // a where the matching half of m is positive, else 0
 __device__ __forceinline__ f2 f2_gate(f2 a, f2 m) { return f2_make(f2_lo(m) > 0.f ? f2_lo(a) : 0.f, f2_hi(m) > 0.f ? f2_hi(a) : 0.f); }

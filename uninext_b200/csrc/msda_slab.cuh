@@ -3,14 +3,13 @@
 // A "slab" is one (batch element, head): the S x 128-byte (fp32) / 64-byte (bf16) strip of value / grad_value that all
 // taps of the pairs (b, *, m) read / update.  These kernels walk the pairs SLAB-MAJOR -- a CTA owns a contiguous range
 // of 64-pair tiles of the (b, m, q) space, i.e. consecutive queries of ONE head -- instead of the memory order
-// (q, m) of msda_tiled.cuh.  That buys two things measured on B200 (profiles/r02b_ubench_smem_rmw_and_egress.txt):
+// (q, m) of msda_tiled.cuh.  That buys two things:
 //
 //   forward  -- the rows gathered by one SM come from one slab whose coarse levels (169 KB at cfg2) stay L1-resident,
-//               and the gather uses 32-byte lanes (LDG.256: 4 lanes per 128-byte row, 8 rows per instruction), which
-//               sustain 119 B/clk/SM from L1 against 80 for LDG.128.
+//               and the gather uses 32-byte lanes (two 16-byte loads: 4 lanes per 128-byte row).
 //   backward -- grad_value traffic is limited by each SM's path into the crossbar (~25 B/clk/SM of red payload, not by
 //               the L2 atomic units).  The coarse levels of the CTA's current slab are therefore accumulated in a
-//               shared-memory WINDOW and leave the SM once, when the CTA moves to another slab.  sm_100a has no fp32
+//               shared-memory WINDOW and leave the SM once, when the CTA moves to another slab.  The SM has no fp32
 //               shared-memory atomic (atomicAdd(float) = CAS loop, 12 cycles per row against 2.1 for a plain
 //               LDS.128 / FFMA / STS.128), so the window is updated WITHOUT atomics under exclusive ownership:
 //               phase P (produce): every group resolves its pair's taps; corners that fall into a window level are
@@ -77,13 +76,11 @@ __device__ __forceinline__ void cta_tile_range(unsigned ntiles, unsigned sms, un
     last = (unsigned)(((unsigned long long)ntiles * (r + 1)) / nr);
 }
 
-// 8 consecutive channels of one row, widened to fp32: one 32-byte (fp32) / 16-byte (bf16) access per lane.
+// 8 consecutive channels of one row, widened to fp32: 32 bytes (fp32) / 16 bytes (bf16) per lane.
 template <typename T> struct Row8;
 template <> struct Row8<float> {
     __device__ static __forceinline__ void load(const unsigned char *p, float (&v)[8]) {
-        asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-                     : "l"(p));
+        RowVec<float, 8>::load(reinterpret_cast<const float *>(p), v);
     }
     __device__ static __forceinline__ void store(float *p, const float (&v)[8]) {
         reinterpret_cast<float4 *>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);

@@ -1,4 +1,4 @@
-// msda_tiled.cuh -- the sm_100a fast path: persistent, row-vectorised gather kernels (forward and backward).
+// msda_tiled.cuh -- the sm_90a fast path: persistent, row-vectorised gather kernels (forward and backward).
 //
 // Thread mapping.  A value row of one head is D contiguous elements; LPR = D / kElems lanes cover it with one 16-byte
 // access each (fp32 D=32: 8 lanes, bf16 D=32: 4 lanes).  A warp therefore carries GPW = 32 / LPR "groups"; each group
@@ -186,7 +186,7 @@ __device__ __forceinline__ float4 masked_weights(const TapGeom &g, float a) {
 // PACKED (bf16 storage, VEC = 8 only): the four corners of a tap are blended in packed bf16 (one HMUL2 + three HFMA2 per
 // 2 channels, corner weights broadcast as bf16x2 in the tap record) and only the blended tap is widened and accumulated in
 // fp32 -- 4 packed ops + 2 widen + 2 adds per word instead of 8 widen + 8 FFMA.  The bf16 forward is issue-bound on exactly
-// that unpack / FFMA stream (smsp__issue_active 68 %, profiles/r01k_enc_bf16_ncu.md).  Costs ~3 bf16 roundings per tap.
+// that unpack / FFMA stream.  Costs ~3 bf16 roundings per tap.
 template <typename T, int VEC, int D, int LP_MAX, int MIN_CTAS, bool TMA, bool SPLIT, bool PACKED = false>
 __global__ void __launch_bounds__(kTiledThreads, MIN_CTAS)
 msda_fwd_tiled(const T *__restrict__ value, const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,

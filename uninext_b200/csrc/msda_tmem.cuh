@@ -1,25 +1,24 @@
-// msda_tmem.cuh -- backward with the coarse levels of grad_value accumulated in TENSOR MEMORY (D = 32, L*P <= 16).
+// msda_tmem.cuh -- backward with the coarse levels of grad_value accumulated in a shared-memory window owned by four
+// consumer warps (D = 32, L*P <= 16).  MSDA_KNOB_SLAB = 2.
 //
-// Why: the backward is bound by each SM's path into the crossbar (~22-25 B/clk/SM of red payload; §5b of DESIGN.md).
-// Combining the coarse levels' contributions inside the SM halves that traffic, but doing it in SHARED memory costs 4 LSU
-// data-pipe wavefronts per row-add on the pipe the gathers already saturate (msda_slab.cuh: -43 % red sectors, +36 % time).
-// Tensor memory has its own port (tcgen05.ld / tcgen05.st, 12-cycle load latency) and is otherwise idle in this kernel.
+// Why: the backward is bound by each SM's path into the crossbar (red.global payload).  Combining the
+// coarse levels' contributions inside the SM halves that traffic.  msda_slab.cuh does it with every warp taking turns
+// as producer and consumer; here the roles are split over dedicated warps so that the gathers never wait for the window.
 //
-// Layout: TMEM is 128 lanes x 512 columns x 32 bit per SM; a warp reaches only the 32 lanes of quadrant (warp % 4).  A
-// window row (32 channels, fp32) is ONE COLUMN of one quadrant: row r -> quadrant r % 4, column r / 4, lane = channel.
-// 4 x 512 columns = 2048 rows: at cfg2 the levels 13x21 and 25x42 (1323 rows) fit.
+// Layout: a window row (32 channels, fp32) is 128 bytes of dynamic shared memory; row r belongs to consumer q = r % 4.
+// The number of rows is what the device's opt-in shared memory leaves after the lists (227 KB on sm_90: 1323 rows, the
+// levels 13x21 and 25x42 of cfg2, fit next to the default lists).
 //
 // Roles (512 threads, one CTA per SM):
 //   warps 0..11  producers -- the msda_bwd_tiled work for 4 pairs each (tap geometry, row gathers, dot products, grad_loc /
 //                grad_attn, red.global for the non-window levels).  Non-zero corners that fall into a window level are
-//                appended to the warp's PRIVATE list for the row's quadrant (positions from ballots: no atomics) and
+//                appended to the warp's PRIVATE list for the row's consumer (positions from ballots: no atomics) and
 //                their weight is cleared in the tap record, which skips the red.global.
-//   warps 12..15 consumers -- warp 12 + q owns quadrant q exclusively: it drains the 12 producer lists of its quadrant
-//                with tcgen05.ld -> FFMA -> tcgen05.st, 8 columns in flight (entries of a batch that repeat a column are
-//                applied afterwards, one by one).  Exclusive ownership = no atomics anywhere.
+//   warps 12..15 consumers -- warp 12 + q owns the rows r % 4 == q exclusively: it drains the 12 producer lists of its
+//                rows with plain shared-memory read-modify-writes (lane = channel).  Exclusive ownership = no atomics.
 //   Lists and the stashed grad_out rows are double-buffered per tile: producers fill buffer t while consumers drain t-1;
 //   one __syncthreads per tile.  When the CTA's tile range moves to another (batch, head) slab, and at the end, the
-//   consumers add their columns to grad_value (red.global.add.f32, one 128-byte row per instruction) and zero them.
+//   consumers add their rows to grad_value (red.global.add.f32, one 128-byte row per instruction) and zero them.
 // A full list falls back to red.global, so capacity never affects the result.
 #pragma once
 
@@ -29,64 +28,39 @@ namespace msda {
 
 constexpr int kTmThreads = 512;
 constexpr int kTmProd = 12;                    // producer warps
-constexpr int kTmCons = 4;                     // consumer warps = TMEM lane quadrants
+constexpr int kTmCons = 4;                     // consumer warps
 constexpr int kTmTile = kTmProd * 4;           // pairs per tile
-constexpr int kTmCols = 512;                   // TMEM columns allocated (all of them: one CTA per SM)
-constexpr int kTmBatch = 8;                    // columns in flight per consumer step
 
-__host__ __device__ inline size_t bwd_tmem_smem_bytes(int list_cap) {
+__host__ __device__ inline size_t bwd_tmem_smem_bytes(int list_cap, int win_rows) {
     return 2 * ((size_t)kTmProd * kTmCons * list_cap * 8        // entry lists
                 + (size_t)kTmProd * kTmCons * 4                 // entry counts
                 + (size_t)kTmTile * 128)                        // grad_out rows of the tile
-           + (size_t)kTmProd * TapSlab<8>::kBytes;               // tap slabs
+           + (size_t)kTmProd * TapSlab<8>::kBytes                // tap slabs
+           + (size_t)win_rows * 128;                             // window
 }
-
-__device__ __forceinline__ void tm_ld(uint32_t taddr, uint32_t &v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr));
-}
-__device__ __forceinline__ void tm_st(uint32_t taddr, uint32_t v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void tm_wait_ld(uint32_t (&v)[kTmBatch]) {      // the registers are only valid after the wait
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]) :: "memory");
-}
-__device__ __forceinline__ void tm_wait_ld1(uint32_t &v) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" : "+r"(v) :: "memory");
-}
-__device__ __forceinline__ void tm_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 template <typename T, int LP_MAX>
 __global__ void __launch_bounds__(kTmThreads, 1)
 msda_bwd_tmem(const T *__restrict__ grad_out, const T *__restrict__ value, const int64_t *__restrict__ shapes,
               const int64_t *__restrict__ lsi, const float *__restrict__ loc, const float *__restrict__ attn,
-              int N, int S, int M, int L, int Lq, int P, int sms, int list_cap,
+              int N, int S, int M, int L, int Lq, int P, int sms, int list_cap, int win_rows,
               float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn)
 {
     constexpr int D = 32, VEC = 4, LPR = 8, NSL = LP_MAX / LPR;
     static_assert(LP_MAX % LPR == 0, "tap capacity must be whole record rounds");
     extern __shared__ __align__(16) unsigned char dyn[];
     __shared__ SlabMap sm;
-    __shared__ uint32_t tmem_slot;
 
-    // dynamic shared memory: [2] lists | [2] counts | [2] g stash | tap slabs
+    // dynamic shared memory: [2] lists | [2] counts | [2] g stash | tap slabs | window
     const size_t list_bytes = (size_t)kTmProd * kTmCons * list_cap * 8;
     uint2 *lists = reinterpret_cast<uint2 *>(dyn);                                        // [buf][warp][quad][cap]
     int *counts = reinterpret_cast<int *>(dyn + 2 * list_bytes);                          // [buf][warp][quad]
     float *gstash = reinterpret_cast<float *>(dyn + 2 * list_bytes + 2 * kTmProd * kTmCons * 4);      // [buf][slot][32]
     unsigned char *slabs = reinterpret_cast<unsigned char *>(gstash) + 2 * (size_t)kTmTile * 128;
+    float *win = reinterpret_cast<float *>(slabs + (size_t)kTmProd * TapSlab<8>::kBytes);     // [row][32]
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    build_slab_map(sm, shapes, lsi, L, N, M, Lq, kTmCons * kTmCols, kTmTile);
-    if (warp == kTmProd) {                       // one warp allocates tensor memory (and frees it at the end)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&tmem_slot)), "r"((unsigned)kTmCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_slot;
+    build_slab_map(sm, shapes, lsi, L, N, M, Lq, win_rows & ~(kTmCons - 1), kTmTile);
     const int wrows = sm.wrows;
     const int LP = L * P;
     const unsigned row_elems = (unsigned)(M * D);
@@ -97,36 +71,25 @@ msda_bwd_tmem(const T *__restrict__ grad_out, const T *__restrict__ value, const
 
     if (warp >= kTmProd) {
         // ======================================= consumers =======================================
-        const int q = warp - kTmProd;                                        // == warp % 4: the quadrant this warp may touch
-        const uint32_t tq = tmem_base + ((uint32_t)(q * 32) << 16);
-        const int ncols = wrows > q ? (wrows - q + 3) / 4 : 0;               // window rows r with r % 4 == q  ->  column r / 4
-        for (int c = 0; c < ncols; ++c) tm_st(tq + (uint32_t)c, 0u);
-        tm_wait_st();
+        const int q = warp - kTmProd;                                        // this warp owns the rows r % 4 == q
+        float *wq = win + q * 32 + lane;                                     // row r = 4 c + q  ->  wq[c * 128]
+        const int ncols = wrows > q ? (wrows - q + 3) / 4 : 0;
+        for (int c = 0; c < ncols; ++c) wq[c * 128] = 0.f;
 
-        auto flush = [&](unsigned sl) {                                       // columns -> grad_value of slab `sl`, then zero
+        auto flush = [&](unsigned sl) {                                       // rows -> grad_value of slab `sl`, then zero
             const int b = (int)(sl / (unsigned)M), m = (int)(sl - (unsigned)b * (unsigned)M);
             float *gslab = grad_value + ((size_t)b * S * M + m) * D + lane;
-            for (int c0 = 0; c0 < ncols; c0 += kTmBatch) {
-                uint32_t v[kTmBatch];
-#pragma unroll
-                for (int j = 0; j < kTmBatch; ++j) { v[j] = 0u; if (c0 + j < ncols) tm_ld(tq + (uint32_t)(c0 + j), v[j]); }
-                tm_wait_ld(v);
-#pragma unroll
-                for (int j = 0; j < kTmBatch; ++j) {
-                    if (c0 + j < ncols) {
-                        const int wr = (c0 + j) * 4 + q;
-                        int row = 0;
-                        for (int l = 0; l < L; ++l) {
-                            const int wb = sm.wbase[l];
-                            if (wb >= 0 && wr >= wb && wr < wb + sm.H[l] * sm.W[l]) row = sm.start[l] + (wr - wb);
-                        }
-                        const float f = __uint_as_float(v[j]);
-                        if (f != 0.f) atomicAdd(gslab + (size_t)row * row_elems, f);          // RED.E.ADD.F32: 128 B per warp
-                        tm_st(tq + (uint32_t)(c0 + j), 0u);
-                    }
+            for (int c = 0; c < ncols; ++c) {
+                const int wr = c * 4 + q;
+                int row = 0;
+                for (int l = 0; l < L; ++l) {
+                    const int wb = sm.wbase[l];
+                    if (wb >= 0 && wr >= wb && wr < wb + sm.H[l] * sm.W[l]) row = sm.start[l] + (wr - wb);
                 }
+                const float f = wq[c * 128];
+                if (f != 0.f) atomicAdd(gslab + (size_t)row * row_elems, f);          // RED.E.ADD.F32: 128 B per warp
+                wq[c * 128] = 0.f;
             }
-            tm_wait_st();
         };
 
         for (unsigned it = 0; it <= ntile; ++it) {
@@ -137,41 +100,10 @@ msda_bwd_tmem(const T *__restrict__ grad_out, const T *__restrict__ value, const
                 for (int w = 0; w < kTmProd; ++w) {
                     const int n = min(counts[(buf * kTmProd + w) * kTmCons + q], list_cap);
                     const uint2 *lst = lists + ((size_t)(buf * kTmProd + w) * kTmCons + q) * list_cap;
-                    for (int i0 = 0; i0 < n; i0 += kTmBatch) {
-                        const int nb = min(kTmBatch, n - i0);
-                        uint32_t col[kTmBatch], acc[kTmBatch];
-                        float wt[kTmBatch], gv[kTmBatch];
-                        unsigned dup = 0;                                     // bit j: entry j repeats the column of an earlier one
-#pragma unroll
-                        for (int j = 0; j < kTmBatch; ++j) {
-                            const uint2 e = j < nb ? lst[i0 + j] : make_uint2(0xffffff00u, 0u);
-                            col[j] = e.x >> 8;
-                            wt[j] = __uint_as_float(e.y);
-                            gv[j] = j < nb ? gs[(e.x & 255u) * 32] : 0.f;
-                            acc[j] = 0u;
-#pragma unroll
-                            for (int k = 0; k < j; ++k) if (j < nb && col[j] == col[k]) dup |= 1u << j;
-                        }
-#pragma unroll
-                        for (int j = 0; j < kTmBatch; ++j) if (j < nb && !((dup >> j) & 1u)) tm_ld(tq + col[j], acc[j]);
-                        tm_wait_ld(acc);
-#pragma unroll
-                        for (int j = 0; j < kTmBatch; ++j)
-                            if (j < nb && !((dup >> j) & 1u))
-                                tm_st(tq + col[j], __float_as_uint(fmaf(wt[j], gv[j], __uint_as_float(acc[j]))));
-                        tm_wait_st();
-                        if (dup) {                                            // rare: same row twice within 8 entries
-#pragma unroll
-                            for (int j = 1; j < kTmBatch; ++j) {
-                                if ((dup >> j) & 1u) {
-                                    uint32_t a = 0u;
-                                    tm_ld(tq + col[j], a);
-                                    tm_wait_ld1(a);
-                                    tm_st(tq + col[j], __float_as_uint(fmaf(wt[j], gv[j], __uint_as_float(a))));
-                                    tm_wait_st();
-                                }
-                            }
-                        }
+                    for (int i = 0; i < n; ++i) {
+                        const uint2 e = lst[i];
+                        float *dst = wq + (size_t)(e.x >> 8) * 128;
+                        *dst = fmaf(__uint_as_float(e.y), gs[(e.x & 255u) * 32], *dst);
                     }
                 }
                 const unsigned sl = tile / sm.tiles_per_slab;
@@ -310,10 +242,6 @@ msda_bwd_tmem(const T *__restrict__ grad_out, const T *__restrict__ value, const
         }
     }
 
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == kTmProd)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((unsigned)kTmCols) : "memory");
 }
 
 }  // namespace msda

