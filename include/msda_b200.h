@@ -44,7 +44,7 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 3   /* 3: sm_90 build; the GEMM timeline diagnostic is gone */
+#define MSDA_ABI_VERSION 4   /* 4: MSDA_KNOB_REGION_BWD */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -80,7 +80,10 @@ uint64_t msda_launch_count(void);
  *   MSDA_KNOB_ZERO_FILL             how msda_backward_* zero-fills grad_value (results identical): 0 = cudaMemsetAsync,
  *                                   1 = msda_zero_fill kernel (16-byte stores, one wave), 2 = the same kernel launched as the
  *                                   programmatic-dependent-launch primary of the tiled backward kernel, whose prologue then
- *                                   overlaps the fill (not while the stream is being captured into a CUDA graph).  Default 2. */
+ *                                   overlaps the fill (not while the stream is being captured into a CUDA graph).  Default 2.
+ *   MSDA_KNOB_REGION_BWD            fp32 backward of encoder self-attention (D = 32, L*P <= 16, Lq == S, large launches):
+ *                                   -1 (auto, default) = msda_bwd_region, which sums grad_value per spatial region in shared
+ *                                   memory before it reaches L2 (msda_region.cuh); 0 = msda_bwd_tiled. */
 #define MSDA_KNOB_SLAB          0
 #define MSDA_KNOB_BWD_WIN_ROWS  1
 #define MSDA_KNOB_BWD_LIST_CAP  2
@@ -91,7 +94,8 @@ uint64_t msda_launch_count(void);
 #define MSDA_KNOB_BF16_PACKED_FWD 7 /* bf16 forward: corners of a tap blended in packed bf16 (HFMA2); 0 / 1            */
 #define MSDA_KNOB_ZERO_FILL     8   /* grad_value zero-fill of the backward: 0 cudaMemsetAsync, 1 own kernel, 2 own kernel
                                        as the PDL primary of the tiled backward kernel (prologue overlaps the fill)   */
-#define MSDA_KNOB_COUNT         9
+#define MSDA_KNOB_REGION_BWD    9   /* fp32 encoder backward: -1 auto = region kernel, 0 = tiled kernel                */
+#define MSDA_KNOB_COUNT         10
 #define MSDA_KNOB_QUERY         (-1000000)
 int msda_set_knob(int knob, int value);
 

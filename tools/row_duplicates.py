@@ -62,7 +62,54 @@ def measure():
     print(f"one (query, head, level), 4 taps x 4 corners: unique/total {uniq / tot:.3f}")
 
 
+def region_estimate(loc0, settings=((8, 2), (8, 3), (8, 4), (8, 6), (12, 4), (16, 4))):
+    """Region tiles of msda_bwd_region (msda_region.cuh), same geometry: tile = (head, R x R region of the finest level),
+    query (x, y) of level l in region floor((x + 0.5) * Wref / W_l / R); window on level l = the region scaled to level l
+    plus `halo` pixels.  Per (R, halo): tiles, max queries per tile, max in-window corner entries per tile, and the
+    row-reds left (corners outside the window + touched window rows per tile) over today's one red per live corner.
+    Ignores the kernel's capacities (stash, entry list, window rows): corners past them red directly."""
+    H = np.array([h for h, _ in shapes]); W = np.array([w for _, w in shapes])
+    Href, Wref = H.max(), W.max()
+    ql = np.repeat(np.arange(len(shapes)), H * W)                     # level / pixel of every query
+    qk = np.arange(S) - starts[ql]
+    qy, qx = qk // W[ql], qk % W[ql]
+    for R, halo in settings:
+        nry, nrx = -(-Href // R), -(-Wref // R)
+        ry = (2 * qy + 1) * Href // (2 * H[ql] * R)
+        rx = (2 * qx + 1) * Wref // (2 * W[ql] * R)
+        reg = ry * nrx + rx
+        nq = np.bincount(reg, minlength=nry * nrx)
+        total = outside = touched = 0
+        max_entries = 0
+        for m in range(loc0.shape[1]):
+            keys, n_in = [], np.zeros(nry * nrx, dtype=np.int64)
+            for l, (Hl, Wl) in enumerate(shapes):
+                x = loc0[:, m, l, :, 0] * Wl - 0.5; y = loc0[:, m, l, :, 1] * Hl - 0.5      # [S, P]
+                inside = (y > -1) & (x > -1) & (y < Hl) & (x < Wl)
+                y0 = np.floor(y).astype(np.int64); x0 = np.floor(x).astype(np.int64)
+                wy0 = np.maximum(0, ry * R * Hl // Href - halo)[:, None]
+                wy1 = np.minimum(Hl, -(-(ry + 1) * R * Hl // Href) + halo)[:, None]
+                wx0 = np.maximum(0, rx * R * Wl // Wref - halo)[:, None]
+                wx1 = np.minimum(Wl, -(-(rx + 1) * R * Wl // Wref) + halo)[:, None]
+                for dy, dx in ((0, 0), (0, 1), (1, 0), (1, 1)):
+                    yy, xx = y0 + dy, x0 + dx
+                    live = inside & (yy >= 0) & (yy < Hl) & (xx >= 0) & (xx < Wl)
+                    inw = live & (yy >= wy0) & (yy < wy1) & (xx >= wx0) & (xx < wx1)
+                    total += live.sum(); outside += (live & ~inw).sum()
+                    r = np.broadcast_to(reg[:, None], inw.shape)[inw]
+                    n_in += np.bincount(r, minlength=nry * nrx)
+                    keys.append(r * S + starts[l] + yy[inw] * Wl + xx[inw])
+            touched += len(np.unique(np.concatenate(keys)))
+            max_entries = max(max_entries, int(n_in.max()))
+        print(f"R={R:2d} halo={halo}: tiles per batch element {nry * nrx} x M, max queries / tile {nq.max()}, "
+              f"max in-window entries / tile {max_entries} ({max_entries * 8 / 1024:.0f} KB), "
+              f"row-reds left / today {(outside + touched) / total:.3f} (outside-window {outside / total:.3f})")
+
+
 for jit in JITTERS:
     loc = make_inputs(cfg1, 'enc', 'cpu', jitter_px=jit)['sampling_locations'][0].numpy()
     print(f"--- jitter {jit} px ---")
     measure()
+    if jit == 2.0:         # the bench's first encoder input: make_inputs(cfg2, "enc", seed=1000), batch element 0
+        print("region tiles, cfg2 seed 1000, batch element 0, all heads:")
+        region_estimate(make_inputs(cfg, 'enc', 'cpu', seed=1000)['sampling_locations'][0].numpy())

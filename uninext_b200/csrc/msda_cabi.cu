@@ -9,6 +9,7 @@
 #include "msda_condinst.cuh"
 #include "msda_generic.cuh"
 #include "msda_module.cuh"
+#include "msda_region.cuh"
 #include "msda_slab.cuh"
 #include "msda_tmem.cuh"
 #include "msda_tiled.cuh"
@@ -69,6 +70,7 @@ struct Knobs {
         v[MSDA_KNOB_BF16_FINE_ROWS].store(env_int("MSDA_BF16_FINE_ROWS", 0));
         v[MSDA_KNOB_BF16_PACKED_FWD].store(env_int("MSDA_BF16_PACKED_FWD", 0));
         v[MSDA_KNOB_ZERO_FILL].store(env_int("MSDA_ZERO_FILL", 2));
+        v[MSDA_KNOB_REGION_BWD].store(env_int("MSDA_REGION_BWD", -1));
     }
 };
 Knobs &knobs() { static Knobs k; return k; }
@@ -205,6 +207,31 @@ cudaError_t launch_fwd(const T *value, const int64_t *shapes, const int64_t *lsi
     return cudaGetLastError();
 }
 
+// Launch of a backward kernel right after the grad_value zero-fill.  When msda_backward_* left t_pdl_next set, the fill
+// kernel just issued on `st` is the programmatic-dependent-launch primary: the backward kernel's prologue overlaps it and
+// the kernel waits for it (pdl_wait_primary) before its first red.
+template <typename K, typename... Args>
+cudaError_t launch_after_fill(K kern, int grid, size_t smem, cudaStream_t st, Args... args) {
+    const bool pdl = t_pdl_next;
+    t_pdl_next = false;
+    if (pdl) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)grid);
+        cfg.blockDim = dim3(msda::kTiledThreads);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+        return e != cudaSuccess ? e : cudaGetLastError();
+    }
+    kern<<<grid, msda::kTiledThreads, smem, st>>>(args...);
+    return cudaGetLastError();
+}
+
 template <typename T, int D, int LP_MAX, int VEC = BwdVec<T>::v>
 cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
                        const float *attn, const Dims &d, float *gv, float *gl, float *ga, cudaStream_t st) {
@@ -224,28 +251,10 @@ cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes,
     const unsigned iter_pairs = msda::kTiledWarps * (split ? 1 : GPW);
     const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;
     const int grid = (int)(tiles_ub < (unsigned)slots ? tiles_ub : (unsigned)slots);
-    const bool pdl = t_pdl_next;
-    t_pdl_next = false;
-    if (pdl) {       // the preceding launch on `st` is msda_zero_fill(grad_value): let this kernel's prologue overlap it
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)grid);
-        cfg.blockDim = dim3(msda::kTiledThreads);
-        cfg.dynamicSmemBytes = 0;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq,
-                                                 d.P, npairs, allow_patches(), gv, gl, ga, (__nv_bfloat16 *)nullptr, 0);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        return e != cudaSuccess ? e : cudaGetLastError();
-    }
-    kern<<<grid, msda::kTiledThreads, 0, st>>>(grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P,
-                                               npairs, allow_patches(), gv, gl, ga, nullptr, 0);
+    const cudaError_t e = launch_after_fill(kern, grid, 0, st, grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L,
+                                            d.Lq, d.P, npairs, allow_patches(), gv, gl, ga, (__nv_bfloat16 *)nullptr, 0);
     g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
+    return e;
 }
 
 // ---- slab-ordered kernels (msda_slab.cuh): D = 32 and L*P <= 16 (every UNINEXT call) ------------------------------
@@ -372,6 +381,37 @@ cudaError_t launch_bwd_tmem(const T *grad_out, const T *value, const int64_t *sh
     return cudaGetLastError();
 }
 
+// ---- region backward (msda_region.cuh): fp32 encoder self-attention, D = 32, L*P <= 16, Lq == S, large launches --------
+// Auto-selected (MSDA_KNOB_REGION_BWD = -1); 0 keeps msda_bwd_tiled.
+bool use_region(const Dims &d) {
+    return knob(MSDA_KNOB_REGION_BWD) != 0 && d.D == 32 && d.L * d.P <= 16 && d.L <= msda::kMaxLevels && d.Lq == d.S &&
+           !use_split((unsigned)((long long)d.N * d.Lq * d.M));
+}
+
+cudaError_t launch_bwd_region(const float *go, const float *value, const int64_t *shapes, const int64_t *lsi,
+                              const float *loc, const float *attn, const Dims &d, float *gv, float *gl, float *ga,
+                              cudaStream_t st) {
+    auto kern = msda::msda_bwd_region<msda::kRegionEdge, msda::kRegionHalo>;
+    constexpr size_t smem = msda::region_smem_bytes();
+    static std::atomic<int> slots_c[kMaxDevices];
+    const int dev = current_device();
+    int slots = slots_c[dev].load(std::memory_order_relaxed);
+    if (slots == 0) {
+        const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        int per_sm = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, msda::kTiledThreads, smem) != cudaSuccess || per_sm < 1)
+            per_sm = 1;
+        slots = per_sm * num_sms();
+        slots_c[dev].store(slots, std::memory_order_relaxed);
+    }
+    const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
+    const cudaError_t e = launch_after_fill(kern, slots, smem, st, go, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq,
+                                            d.P, npairs, gv, gl, ga);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return e;
+}
+
 #define MSDA_ROUTE_LP(T, DD, CALL)                                   \
     (LP <= 16 ? CALL<T, DD, 16> : CALL<T, DD, 32>)
 
@@ -407,6 +447,7 @@ cudaError_t bwd_fast(const T *go, const T *value, const int64_t *shapes, const i
         if (knob(MSDA_KNOB_F32_VEC8_BWD) == 1 && LP <= 16 && d.D == 32 &&
             !((reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(go)) & 31u))
             return launch_bwd<T, 32, 16, 8>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+        if (use_region(d)) return launch_bwd_region(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
     }
     switch (d.D) {
         case 16: if constexpr (sizeof(T) == 4) return MSDA_ROUTE_LP(T, 16, launch_bwd)(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st); break;

@@ -1,0 +1,345 @@
+// msda_region.cuh -- fp32 encoder backward (D = 32, L*P <= 16, Lq == S) that sums grad_value contributions per spatial
+// region on chip and sends each touched row to L2 once.
+//
+// msda_bwd_tiled issues one 16-byte red.global per lane and live corner: a 128-byte row-add per corner, ~20 M of them per
+// cfg2 encoder call, 8x the compulsory grad_value bytes.  In encoder self-attention the queries ARE the pixels of the
+// pyramid and every query samples within a few pixels of its own position on every level.  So a CTA that takes all
+// queries of one (batch, head) whose pixel centre lies in one R x R region of the finest level touches only a small
+// rectangle ("window") of each level, and it can add those contributions up on chip first.
+//
+// Tile = (b, m, region).  A query at pixel (x, y) of level l belongs to region floor((x + 0.5) * Wref / W_l / R) in x (likewise
+// in y; Wref / Href = the largest level), so a region holds one contiguous x-range and y-range per level, in closed form.
+// The window on level l is the region scaled to level l plus kRegionHalo pixels.  Per tile:
+//   phase A (one 8-lane group per pair, as msda_bwd_tiled): gathers, grad_loc / grad_attn epilogue unchanged.  The pair's
+//            grad_out row is stashed in shared memory; a non-zero corner inside the window becomes an entry {window row,
+//            coefficient} at the fixed position (slot, tap, corner) -- no atomics on the gather path.  A corner outside the
+//            window, or of a query past the stash, reds directly as in msda_bwd_tiled, so the capacities never change a
+//            result.
+//   phase B: counting sort of the entries by window row (integer shared atomics only: fp32 shared atomics are CAS loops)
+//            into {coefficient, slot} arrays.
+//   phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
+// A level table that does not tile [0, S) (the patch-order condition) runs in linear chunks of pairs with no window.
+#pragma once
+
+#include "msda_tiled.cuh"
+
+namespace msda {
+
+constexpr int kRegionEdge = 8;            // region edge, in pixels of the finest level
+constexpr int kRegionHalo = 4;            // window margin around the scaled region, in pixels of each level
+constexpr int kRegionSlots = 96;          // queries per tile whose grad_out row is stashed (the rest red directly)
+constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past this budget red directly)
+constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
+constexpr int kRegionMinCtas = 2;
+constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
+
+// entry rows (u16) + entry coefficients + sorted coefficients (f32) + sorted slots (u8) + grad_out stash + row counts
+constexpr size_t region_smem_bytes() {
+    return (size_t)kRegionEntries * (2 + 4 + 4 + 1) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4;
+}
+
+struct RegionMap {
+    int H[kMaxLevels], W[kMaxLevels], start[kMaxLevels];
+    int Href, Wref, nry, nrx;
+    int region;                 // 1: region tiles; 0: linear chunks of kRegionIterSlots pairs, no window
+    unsigned ntiles;
+};
+
+struct RegionTile {
+    int b, m, nq, nwin;
+    unsigned base_pair;         // linear chunks
+    int qy0[kMaxLevels], qx0[kMaxLevels], qny[kMaxLevels], qnx[kMaxLevels], qpre[kMaxLevels + 1];
+    int wy0[kMaxLevels], wx0[kMaxLevels], wh[kMaxLevels], ww[kMaxLevels], wbase[kMaxLevels + 1];
+};
+
+// Per-warp window records, laid out like TapSlab's row records: {window row of corner 00, (dy * ww) << 5 | dw << 4 | mask}.
+template <int LPR>
+struct WinSlab {
+    static constexpr int kStride = LPR * 8 + 8;
+    static constexpr int kBytes = (32 / LPR) * kStride;
+    int2 *p;
+    __device__ __forceinline__ WinSlab(unsigned char *warp_base, int grp)
+        : p(reinterpret_cast<int2 *>(warp_base + grp * kStride)) {}
+    __device__ __forceinline__ void put(int j, int2 v) { p[j] = v; }
+    __device__ __forceinline__ int2 get(int j) const { return p[j]; }
+};
+
+// First pixel of a level of n pixels (reference extent `ref`) whose region index is >= r.
+__device__ __forceinline__ int region_first(int r, int n, int ref, int R) {
+    const long long num = 2ll * r * n * R - ref;
+    return num <= 0 ? 0 : (int)min((long long)n, (num + 2ll * ref - 1) / (2ll * ref));
+}
+
+template <int R, int HALO>
+__global__ void __launch_bounds__(kTiledThreads, kRegionMinCtas)
+msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ value,
+                const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
+                const float *__restrict__ loc, const float *__restrict__ attn,
+                int N, int S, int M, int L, int Lq, int P, unsigned npairs,
+                float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn)
+{
+    constexpr int D = 32, VEC = 4, LPR = D / VEC, GPW = 32 / LPR, LP_MAX = 16, NSL = LP_MAX / LPR;
+    static_assert(GPW * kTiledWarps == kRegionIterSlots && kRegionSlots <= 256 && kRegionWinRows < 0xffff &&
+                  kRegionSlots % kRegionIterSlots == 0, "entry layout");
+    constexpr unsigned short kNoRow = 0xffff;
+
+    __shared__ RegionMap rm;
+    __shared__ RegionTile tl;
+    __shared__ int wsum[kTiledWarps];
+    __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<LPR>::kBytes];
+    __shared__ __align__(16) unsigned char win_mem[kTiledWarps * WinSlab<LPR>::kBytes];
+    extern __shared__ __align__(16) unsigned char dyn[];
+    float *e_coef = reinterpret_cast<float *>(dyn);                                   // [slot][tap][corner]
+    float *s_coef = e_coef + kRegionEntries;                                          // sorted by window row
+    float4 *gstash = reinterpret_cast<float4 *>(s_coef + kRegionEntries);             // [slot][lane] grad_out slices
+    int *cnt = reinterpret_cast<int *>(gstash + kRegionSlots * LPR);                  // [window row]
+    unsigned short *e_row = reinterpret_cast<unsigned short *>(cnt + kRegionWinRows); // [slot][tap][corner], kNoRow = none
+    unsigned char *s_slot = reinterpret_cast<unsigned char *>(e_row + kRegionEntries);
+
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane % LPR, grp = lane / LPR;
+    const int LP = L * P;
+    const unsigned row_elems = (unsigned)(M * D);
+    TapSlab<LPR> slab(slab_mem + warp * TapSlab<LPR>::kBytes, grp);
+    WinSlab<LPR> win(win_mem + warp * WinSlab<LPR>::kBytes, grp);
+
+    if (threadIdx.x == 0) {            // the map comes from the device-resident level table: no host read, capture-safe
+        int run = 0, href = 0, wref = 0;
+        bool tiled = (Lq == S);
+        for (int l = 0; l < L; ++l) {
+            const int h = (int)shapes[2 * l], w = (int)shapes[2 * l + 1], st = (int)lsi[l];
+            rm.H[l] = h; rm.W[l] = w; rm.start[l] = st;
+            tiled = tiled && (st == run) && h > 0 && w > 0;
+            run += h * w;
+            href = max(href, h); wref = max(wref, w);
+        }
+        tiled = tiled && (run == S);
+        rm.region = tiled ? 1 : 0;
+        rm.Href = href; rm.Wref = wref;
+        rm.nry = (href + R - 1) / R; rm.nrx = (wref + R - 1) / R;
+        rm.ntiles = tiled ? (unsigned)N * (unsigned)M * (unsigned)(rm.nry * rm.nrx)
+                          : (npairs + kRegionIterSlots - 1) / kRegionIterSlots;
+    }
+    __syncthreads();
+    pdl_wait_primary();      // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
+
+    for (unsigned tile = blockIdx.x; tile < rm.ntiles; tile += gridDim.x) {
+        // ---- tile geometry: thread l resolves level l, thread 0 then lays the levels out ----
+        if (rm.region) {
+            const int m = (int)(tile % (unsigned)M);         // heads fastest: concurrent tiles share loc / attn pages
+            const unsigned r = tile / (unsigned)M, per_b = (unsigned)(rm.nry * rm.nrx);
+            const int reg = (int)(r % per_b), ry = reg / rm.nrx, rx = reg % rm.nrx;
+            const int l = threadIdx.x;
+            if (l < L) {
+                const int H = rm.H[l], W = rm.W[l];
+                const int y0 = region_first(ry, H, rm.Href, R), y1 = region_first(ry + 1, H, rm.Href, R);
+                const int x0 = region_first(rx, W, rm.Wref, R), x1 = region_first(rx + 1, W, rm.Wref, R);
+                tl.qy0[l] = y0; tl.qny[l] = y1 - y0; tl.qx0[l] = x0; tl.qnx[l] = x1 - x0;
+                const int wy0 = max(0, (int)((long long)ry * R * H / rm.Href) - HALO);
+                const int wy1 = min(H, (int)(((long long)(ry + 1) * R * H + rm.Href - 1) / rm.Href) + HALO);
+                const int wx0 = max(0, (int)((long long)rx * R * W / rm.Wref) - HALO);
+                const int wx1 = min(W, (int)(((long long)(rx + 1) * R * W + rm.Wref - 1) / rm.Wref) + HALO);
+                tl.wy0[l] = wy0; tl.wh[l] = wy1 - wy0; tl.wx0[l] = wx0; tl.ww[l] = wx1 - wx0;
+            }
+            if (threadIdx.x == 0) { tl.m = m; tl.b = (int)(r / per_b); }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                int nq = 0, nw = 0;
+                for (int k = 0; k < L; ++k) {
+                    tl.qpre[k] = nq; nq += tl.qny[k] * tl.qnx[k];
+                    const int rows = tl.wh[k] * tl.ww[k];
+                    if (nw + rows > kRegionWinRows) { tl.wh[k] = tl.ww[k] = 0; }     // over budget: this level reds directly
+                    tl.wbase[k] = nw; nw += tl.wh[k] * tl.ww[k];
+                }
+                tl.qpre[L] = nq; tl.wbase[L] = nw;
+                tl.nq = nq; tl.nwin = nw;
+            }
+        } else if (threadIdx.x == 0) {
+            tl.base_pair = tile * kRegionIterSlots;
+            tl.nq = (int)min((unsigned)kRegionIterSlots, npairs - tl.base_pair);
+            tl.nwin = 0;
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < tl.nwin; i += kTiledThreads) cnt[i] = 0;
+
+        // ---- phase A: gathers, grad_loc / grad_attn; in-window corners become entries, the others red ----
+#pragma unroll 1
+        for (int it = 0; it * kRegionIterSlots < tl.nq; ++it) {
+            const int slot = it * kRegionIterSlots + warp * GPW + grp;
+            const bool active = slot < tl.nq;
+            unsigned pair = 0; int b = 0, m = 0;
+            if (active) {
+                if (rm.region) {
+                    int l = 0;
+                    while (l + 1 < L && slot >= tl.qpre[l + 1]) ++l;
+                    const int k = slot - tl.qpre[l], y = tl.qy0[l] + k / tl.qnx[l], x = tl.qx0[l] + k % tl.qnx[l];
+                    b = tl.b; m = tl.m;
+                    pair = ((unsigned)b * (unsigned)Lq + (unsigned)(rm.start[l] + y * rm.W[l] + x)) * (unsigned)M + (unsigned)m;
+                } else {
+                    pair = tl.base_pair + (unsigned)slot;
+                    m = (int)(pair % (unsigned)M);
+                    b = (int)((pair / (unsigned)M) / (unsigned)Lq);
+                }
+            }
+            const bool stash = rm.region && active && slot < kRegionSlots;        // group-uniform
+
+            float g[VEC] = {0.f, 0.f, 0.f, 0.f};
+            if (active) RowVec<float, VEC>::load(grad_out + (size_t)pair * D + (size_t)sub * VEC, g);
+            if (stash) gstash[slot * LPR + sub] = make_float4(g[0], g[1], g[2], g[3]);
+
+            // ---- stage 1: this lane resolves taps sub, sub + LPR (dead taps: zero weight, row 0, no window) ----
+            float4 tw[NSL];
+            int2 tr[NSL], twin[NSL];
+            float tlh[NSL], tlw[NSL], ta[NSL];
+            unsigned tmeta[NSL];
+#pragma unroll
+            for (int k = 0; k < NSL; ++k) {
+                const int s = sub + k * LPR;
+                tw[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+                tr[k] = twin[k] = make_int2(0, 0);
+                tlh[k] = tlw[k] = ta[k] = 0.f; tmeta[k] = 0;
+                if (s < LP && active) {
+                    const size_t t = (size_t)pair * LP + s;
+                    const float2 xy = __ldg(reinterpret_cast<const float2 *>(loc) + t);
+                    const float a = __ldg(attn + t);
+                    const int l = s / P;
+                    const TapGeom gm = tap_geometry(xy.x, xy.y, rm.H[l], rm.W[l], rm.start[l]);
+                    tw[k] = masked_weights(gm, a);
+                    tr[k] = make_int2(gm.r0, gm.r1 | (gm.dw << 31));
+                    tlh[k] = gm.lh; tlw[k] = gm.lw; ta[k] = a; tmeta[k] = gm.mask | ((unsigned)l << 4);
+                    if (stash) {
+                        const int W = rm.W[l], o0 = gm.r0 - rm.start[l], o1 = gm.r1 - rm.start[l];
+                        const int y0 = o0 / W, x0 = o0 - y0 * W, y1 = o1 / W;
+                        const int wwl = tl.ww[l], whl = tl.wh[l];
+                        const int ry0 = y0 - tl.wy0[l], ry1 = y1 - tl.wy0[l], rx0 = x0 - tl.wx0[l], rx1 = rx0 + gm.dw;
+                        const unsigned iy0 = (unsigned)ry0 < (unsigned)whl, iy1 = (unsigned)ry1 < (unsigned)whl;
+                        const unsigned ix0 = (unsigned)rx0 < (unsigned)wwl, ix1 = (unsigned)rx1 < (unsigned)wwl;
+                        const unsigned inwin = (iy0 & ix0) | ((iy0 & ix1) << 1) | ((iy1 & ix0) << 2) | ((iy1 & ix1) << 3);
+                        twin[k] = make_int2(tl.wbase[l] + ry0 * wwl + rx0, (((y1 - y0) * wwl) << 5) | (gm.dw << 4) | (int)inwin);
+                    }
+                }
+            }
+
+            const size_t slab_off = ((size_t)b * S * M + m) * D + (size_t)sub * VEC;
+            const float *base = value + slab_off;
+            float *gbase = grad_value + slab_off;
+
+            // ---- stage 2 ----
+#pragma unroll
+            for (int k = 0; k < NSL; ++k) {
+                __syncwarp();
+                slab.put(sub, tw[k], tr[k]);
+                win.put(sub, twin[k]);
+                __syncwarp();
+                float part[LPR][4];
+#pragma unroll
+                for (int j = 0; j < LPR; ++j) {
+                    const float4 w4 = slab.weights(j);
+                    const int2 rr = slab.rows(j);
+                    const int2 wi = win.get(j);
+                    const float w[4] = {w4.x, w4.y, w4.z, w4.w};
+                    const unsigned nz = (unsigned)(w4.x != 0.f) | ((unsigned)(w4.y != 0.f) << 1) |
+                                        ((unsigned)(w4.z != 0.f) << 2) | ((unsigned)(w4.w != 0.f) << 3);
+                    const unsigned ok = (unsigned)wi.y & nz & 15u;          // corners that become entries (group-uniform)
+                    if (stash && sub < 4) {                                   // lane c files corner c of tap j
+                        const int dw = (wi.y >> 4) & 1, dhw = wi.y >> 5;
+                        const int wrow = wi.x + ((sub & 1) ? dw : 0) + ((sub & 2) ? dhw : 0);
+                        const int e = ((slot * LP_MAX + k * LPR + j) << 2) + sub;
+                        e_row[e] = ((ok >> sub) & 1u) ? (unsigned short)wrow : kNoRow;
+                        e_coef[e] = sub == 0 ? w4.x : sub == 1 ? w4.y : sub == 2 ? w4.z : w4.w;
+                    }
+                    const unsigned dwo = (rr.y < 0) ? row_elems : 0u;
+                    unsigned long long off[4];
+                    off[0] = (unsigned long long)(unsigned)rr.x * row_elems;
+                    off[1] = off[0] + dwo;
+                    off[2] = (unsigned long long)(unsigned)(rr.y & 0x7fffffff) * row_elems;
+                    off[3] = off[2] + dwo;
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        float v[VEC];
+                        RowVec<float, VEC>::load(base + off[c], v);
+                        float dsum = 0.f;
+#pragma unroll
+                        for (int e = 0; e < VEC; ++e) dsum = fmaf(g[e], v[e], dsum);
+                        part[j][c] = dsum;
+                        if (w[c] != 0.f && !((ok >> c) & 1u))
+                            red_add_v4(gbase + off[c], w[c] * g[0], w[c] * g[1], w[c] * g[2], w[c] * g[3]);
+                    }
+                }
+                float dot[4];
+                group_reduce_scatter<LPR>(part, sub, dot);
+                const int s = sub + k * LPR;
+                if (s < LP && active) {
+                    const int l = (int)(tmeta[k] >> 4);
+                    finish_tap(dot, tmeta[k], tlh[k], tlw[k], ta[k], rm.H[l], rm.W[l], (size_t)pair * LP + s, grad_loc,
+                               grad_attn);
+                }
+            }
+        }
+
+        const int nwin = tl.nwin;
+        if (nwin > 0) {
+            __syncthreads();
+            const int n = min(tl.nq, kRegionSlots) * LP_MAX * 4;
+            // ---- phase B: counting sort of the entries by window row ----
+            for (int e = threadIdx.x; e < n; e += kTiledThreads) {
+                const unsigned short r = e_row[e];
+                if (r != kNoRow) atomicAdd(&cnt[r], 1);
+            }
+            __syncthreads();
+            {   // exclusive scan of cnt[0, nwin): 4 rows per thread
+                const int i0 = threadIdx.x * 4;
+                int c[4], sum = 0;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) { c[q] = (i0 + q < nwin) ? cnt[i0 + q] : 0; sum += c[q]; }
+                int incl = sum;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const int t = __shfl_up_sync(kFullMask, incl, d);
+                    if (lane >= d) incl += t;
+                }
+                if (lane == 31) wsum[warp] = incl;
+                __syncthreads();
+                int run = incl - sum;
+                for (int w = 0; w < warp; ++w) run += wsum[w];
+#pragma unroll
+                for (int q = 0; q < 4; ++q)
+                    if (i0 + q < nwin) { cnt[i0 + q] = run; run += c[q]; }
+            }
+            static_assert(kRegionWinRows <= 4 * kTiledThreads, "scan covers 4 rows per thread");
+            __syncthreads();
+            for (int e = threadIdx.x; e < n; e += kTiledThreads) {
+                const unsigned short r = e_row[e];
+                if (r != kNoRow) {
+                    const int pos = atomicAdd(&cnt[r], 1);
+                    s_coef[pos] = e_coef[e];
+                    s_slot[pos] = (unsigned char)(e / (LP_MAX * 4));
+                }
+            }
+            __syncthreads();          // bucket r is now [r ? cnt[r - 1] : 0, cnt[r]) of s_coef / s_slot
+
+            // ---- phase C: one group per touched row, one red per lane ----
+            const int b = tl.b, m = tl.m;
+            for (int r = warp * GPW + grp; r < nwin; r += kRegionIterSlots) {
+                const int beg = r ? cnt[r - 1] : 0, end = cnt[r];
+                if (beg == end) continue;
+                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+                for (int i = beg; i < end; ++i) {
+                    const float cf = s_coef[i];
+                    const float4 gs = gstash[s_slot[i] * LPR + sub];
+                    acc.x = fmaf(cf, gs.x, acc.x); acc.y = fmaf(cf, gs.y, acc.y);
+                    acc.z = fmaf(cf, gs.z, acc.z); acc.w = fmaf(cf, gs.w, acc.w);
+                }
+                int l = 0;
+                while (l + 1 < L && r >= tl.wbase[l + 1]) ++l;
+                const int k = r - tl.wbase[l], y = tl.wy0[l] + k / tl.ww[l], x = tl.wx0[l] + k % tl.ww[l];
+                const int row = rm.start[l] + y * rm.W[l] + x;
+                red_add_v4(grad_value + (((size_t)b * S + row) * M + m) * D + (size_t)sub * VEC, acc.x, acc.y, acc.z, acc.w);
+            }
+        }
+        __syncthreads();              // the next tile rewrites tl, the entry list, the stash and the counts
+    }
+}
+
+}  // namespace msda

@@ -376,6 +376,21 @@ __device__ __forceinline__ void group_reduce_scatter(float (&part)[LPR][4], int 
     for (int c = 0; c < 4; ++c) res[c] = part[0][c];
 }
 
+// The lane that resolved tap t finishes it from the four corner dot products dot_k = sum_c g[c] * V_k[c]:
+//   grad_attn[t] = sum_k w_k dot_k ;  grad_loc[t] = (W_l * a * d/dlw, H_l * a * d/dlh)  (bilinear weights without a).
+// mk = corner mask | level << 4 (corners outside the map contribute nothing).
+__device__ __forceinline__ void finish_tap(const float (&dot)[4], unsigned mk, float lh, float lw, float a, int H, int W,
+                                           size_t t, float *__restrict__ grad_loc, float *__restrict__ grad_attn) {
+    const float d0 = (mk & 1u) ? dot[0] : 0.f, d1 = (mk & 2u) ? dot[1] : 0.f;
+    const float d2 = (mk & 4u) ? dot[2] : 0.f, d3 = (mk & 8u) ? dot[3] : 0.f;
+    const float hh = 1.f - lh, hw = 1.f - lw;
+    const float val = hh * hw * d0 + hh * lw * d1 + lh * hw * d2 + lh * lw * d3;   // cuh:155-156
+    const float gw = hh * (d1 - d0) + lh * (d3 - d2);                               // cuh:124,133,142,151
+    const float gh = hw * (d2 - d0) + lw * (d3 - d1);                               // cuh:123,132,141,150
+    grad_attn[t] = val;
+    reinterpret_cast<float2 *>(grad_loc)[t] = make_float2((float)W * a * gw, (float)H * a * gh);      // cuh:157-158
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // backward (reference cuh:87-159 + cuh:301-403):
 //   grad_value[corner rows] += w_corner * a * g            (16-byte vector reductions, fp32 accumulator)
@@ -545,19 +560,9 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
                 // ---- the lane that resolved the tap finishes it ----
                 const int s = SPLIT ? grp * TPG + sub : sub + k * LPR;
                 if ((!SPLIT || sub < TPG) && s < LP && active) {
-                    const unsigned mk = tmeta[k];
-                    const int l = (int)(mk >> 4);
-                    const float d0 = (mk & 1u) ? dot[0] : 0.f, d1 = (mk & 2u) ? dot[1] : 0.f;
-                    const float d2 = (mk & 4u) ? dot[2] : 0.f, d3 = (mk & 8u) ? dot[3] : 0.f;
-                    const float lh = tlh[k], lw = tlw[k], hh = 1.f - lh, hw = 1.f - lw;
-                    const float val = hh * hw * d0 + hh * lw * d1 + lh * hw * d2 + lh * lw * d3;   // cuh:155-156
-                    const float gw = hh * (d1 - d0) + lh * (d3 - d2);                               // cuh:124,133,142,151
-                    const float gh = hw * (d2 - d0) + lw * (d3 - d1);                               // cuh:123,132,141,150
-                    const size_t t = (size_t)pair * LP + s;
-                    grad_attn[t] = val;
-                    const float a = ta[k];
-                    reinterpret_cast<float2 *>(grad_loc)[t] =
-                        make_float2((float)wm.W[l] * a * gw, (float)wm.H[l] * a * gh);              // cuh:157-158
+                    const int l = (int)(tmeta[k] >> 4);
+                    finish_tap(dot, tmeta[k], tlh[k], tlw[k], ta[k], wm.H[l], wm.W[l], (size_t)pair * LP + s, grad_loc,
+                               grad_attn);
                 }
             }
         }
