@@ -10,13 +10,17 @@
 // Tile = (b, m, region).  A query at pixel (x, y) of level l belongs to region floor((x + 0.5) * Wref / W_l / R) in x (likewise
 // in y; Wref / Href = the largest level), so a region holds one contiguous x-range and y-range per level, in closed form.
 // The window on level l is the region scaled to level l plus kRegionHalo pixels.  Per tile:
-//   phase A (one 8-lane group per pair, as msda_bwd_tiled): gathers, grad_loc / grad_attn epilogue unchanged.  The pair's
-//            grad_out row is stashed in shared memory; a non-zero corner inside the window becomes an entry {window row,
-//            coefficient} at the fixed position (slot, tap, corner) -- no atomics on the gather path.  A corner outside the
-//            window, or of a query past the stash, reds directly as in msda_bwd_tiled, so the capacities never change a
-//            result.
+//   staging: the value rows of the window's last levels (the coarsest of a feature pyramid, whose rows are gathered most
+//            often) are copied into shared memory with 16-byte cp.async, from the last level down while they fit
+//            kRegionStageRows.  The staged rows are a suffix [sfirst, nwin) of the window-row numbering.
+//   phase A (one 8-lane group per pair, as msda_bwd_tiled): gathers, grad_loc / grad_attn epilogue unchanged; a corner
+//            inside a staged level is read from shared memory, every other corner from global memory (same values, same
+//            FMA order).  The pair's grad_out row is stashed in shared memory; a non-zero corner inside the window
+//            becomes an entry {window row, coefficient} at the fixed position (slot, tap, corner) -- no atomics on the
+//            gather path.  A corner outside the window, or of a query past the stash, reds directly as in
+//            msda_bwd_tiled, so the capacities never change a result.
 //   phase B: counting sort of the entries by window row (integer shared atomics only: fp32 shared atomics are CAS loops)
-//            into {coefficient, slot} arrays.
+//            into {coefficient, slot} arrays, which overlay the staged rows (dead once phase A is done).
 //   phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
 // A level table that does not tile [0, S) (the patch-order condition) runs in linear chunks of pairs with no window.
 #pragma once
@@ -29,14 +33,23 @@ constexpr int kRegionEdge = 8;            // region edge, in pixels of the fines
 constexpr int kRegionHalo = 4;            // window margin around the scaled region, in pixels of each level
 constexpr int kRegionSlots = 96;          // queries per tile whose grad_out row is stashed (the rest red directly)
 constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past this budget red directly)
+constexpr int kRegionStageRows = 384;     // window rows staged in shared memory (cfg2: levels 1-3, at most 366 rows)
 constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
 constexpr int kRegionMinCtas = 2;
 constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
 
-// entry rows (u16) + entry coefficients + sorted coefficients (f32) + sorted slots (u8) + grad_out stash + row counts
+// entry coefficients (f32) + grad_out stash + row counts + entry rows (u16) + the larger of the staged value rows and
+// the sorted {coefficient (f32), slot (u8)} arrays, which share their space
 constexpr size_t region_smem_bytes() {
-    return (size_t)kRegionEntries * (2 + 4 + 4 + 1) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4;
+    constexpr size_t staged = (size_t)kRegionStageRows * 128, sorted = (size_t)kRegionEntries * (4 + 1);
+    return (size_t)kRegionEntries * (4 + 2) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4 +
+           (staged > sorted ? staged : sorted);
 }
+
+__device__ __forceinline__ void cp_async16(void *dst, const void *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 struct RegionMap {
     int H[kMaxLevels], W[kMaxLevels], start[kMaxLevels];
@@ -47,12 +60,14 @@ struct RegionMap {
 
 struct RegionTile {
     int b, m, nq, nwin;
+    int sfirst;                 // first staged window row: rows [sfirst, nwin) are in shared memory
     unsigned base_pair;         // linear chunks
     int qy0[kMaxLevels], qx0[kMaxLevels], qny[kMaxLevels], qnx[kMaxLevels], qpre[kMaxLevels + 1];
     int wy0[kMaxLevels], wx0[kMaxLevels], wh[kMaxLevels], ww[kMaxLevels], wbase[kMaxLevels + 1];
 };
 
-// Per-warp window records, laid out like TapSlab's row records: {window row of corner 00, (dy * ww) << 5 | dw << 4 | mask}.
+// Per-warp window records, laid out like TapSlab's row records:
+// {window row of corner 00, (dy * ww) << 6 | staged level << 5 | dw << 4 | in-window corner mask}.
 template <int LPR>
 struct WinSlab {
     static constexpr int kStride = LPR * 8 + 8;
@@ -90,11 +105,12 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
     __shared__ __align__(16) unsigned char win_mem[kTiledWarps * WinSlab<LPR>::kBytes];
     extern __shared__ __align__(16) unsigned char dyn[];
     float *e_coef = reinterpret_cast<float *>(dyn);                                   // [slot][tap][corner]
-    float *s_coef = e_coef + kRegionEntries;                                          // sorted by window row
-    float4 *gstash = reinterpret_cast<float4 *>(s_coef + kRegionEntries);             // [slot][lane] grad_out slices
+    float4 *gstash = reinterpret_cast<float4 *>(e_coef + kRegionEntries);             // [slot][lane] grad_out slices
     int *cnt = reinterpret_cast<int *>(gstash + kRegionSlots * LPR);                  // [window row]
     unsigned short *e_row = reinterpret_cast<unsigned short *>(cnt + kRegionWinRows); // [slot][tap][corner], kNoRow = none
-    unsigned char *s_slot = reinterpret_cast<unsigned char *>(e_row + kRegionEntries);
+    float4 *vstage = reinterpret_cast<float4 *>(e_row + kRegionEntries);              // phase A: [staged row][lane]
+    float *s_coef = reinterpret_cast<float *>(vstage);                                // phases B, C: sorted by window row
+    unsigned char *s_slot = reinterpret_cast<unsigned char *>(s_coef + kRegionEntries);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane % LPR, grp = lane / LPR;
@@ -153,14 +169,29 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                 }
                 tl.qpre[L] = nq; tl.wbase[L] = nw;
                 tl.nq = nq; tl.nwin = nw;
+                int sf = nw;               // stage whole levels from the last one down while they fit
+                for (int k = L - 1; k >= 0 && nw - tl.wbase[k] <= kRegionStageRows; --k) sf = tl.wbase[k];
+                tl.sfirst = sf;
             }
         } else if (threadIdx.x == 0) {
             tl.base_pair = tile * kRegionIterSlots;
             tl.nq = (int)min((unsigned)kRegionIterSlots, npairs - tl.base_pair);
-            tl.nwin = 0;
+            tl.nwin = tl.sfirst = 0;
         }
         __syncthreads();
+        // ---- staging: window rows [sfirst, nwin), one 16-byte cp.async per lane and row slice ----
+        const int sfirst = tl.sfirst;
+        for (int i = threadIdx.x; i < (tl.nwin - sfirst) * LPR; i += kTiledThreads) {
+            const int r = sfirst + i / LPR;
+            int l = L - 1;
+            while (r < tl.wbase[l]) --l;
+            const int k = r - tl.wbase[l], y = tl.wy0[l] + k / tl.ww[l], x = tl.wx0[l] + k % tl.ww[l];
+            const int row = rm.start[l] + y * rm.W[l] + x;
+            cp_async16(vstage + i, value + (((size_t)tl.b * S + row) * M + tl.m) * D + (size_t)(i % LPR) * VEC);
+        }
         for (int i = threadIdx.x; i < tl.nwin; i += kTiledThreads) cnt[i] = 0;
+        cp_async_wait_all();
+        __syncthreads();
 
         // ---- phase A: gathers, grad_loc / grad_attn; in-window corners become entries, the others red ----
 #pragma unroll 1
@@ -207,7 +238,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                     tw[k] = masked_weights(gm, a);
                     tr[k] = make_int2(gm.r0, gm.r1 | (gm.dw << 31));
                     tlh[k] = gm.lh; tlw[k] = gm.lw; ta[k] = a; tmeta[k] = gm.mask | ((unsigned)l << 4);
-                    if (stash) {
+                    if (rm.region) {
                         const int W = rm.W[l], o0 = gm.r0 - rm.start[l], o1 = gm.r1 - rm.start[l];
                         const int y0 = o0 / W, x0 = o0 - y0 * W, y1 = o1 / W;
                         const int wwl = tl.ww[l], whl = tl.wh[l];
@@ -215,7 +246,9 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                         const unsigned iy0 = (unsigned)ry0 < (unsigned)whl, iy1 = (unsigned)ry1 < (unsigned)whl;
                         const unsigned ix0 = (unsigned)rx0 < (unsigned)wwl, ix1 = (unsigned)rx1 < (unsigned)wwl;
                         const unsigned inwin = (iy0 & ix0) | ((iy0 & ix1) << 1) | ((iy1 & ix0) << 2) | ((iy1 & ix1) << 3);
-                        twin[k] = make_int2(tl.wbase[l] + ry0 * wwl + rx0, (((y1 - y0) * wwl) << 5) | (gm.dw << 4) | (int)inwin);
+                        const int staged = tl.wbase[l] >= tl.sfirst;
+                        twin[k] = make_int2(tl.wbase[l] + ry0 * wwl + rx0,
+                                            (((y1 - y0) * wwl) << 6) | (staged << 5) | (gm.dw << 4) | (int)inwin);
                     }
                 }
             }
@@ -240,9 +273,11 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                     const float w[4] = {w4.x, w4.y, w4.z, w4.w};
                     const unsigned nz = (unsigned)(w4.x != 0.f) | ((unsigned)(w4.y != 0.f) << 1) |
                                         ((unsigned)(w4.z != 0.f) << 2) | ((unsigned)(w4.w != 0.f) << 3);
-                    const unsigned ok = (unsigned)wi.y & nz & 15u;          // corners that become entries (group-uniform)
+                    // corners that become entries / that are read from the staged rows (both group-uniform)
+                    const unsigned ok = stash ? (unsigned)wi.y & nz & 15u : 0u;
+                    const unsigned sm = (wi.y & 32) ? (unsigned)wi.y & 15u : 0u;
+                    const int dw = (wi.y >> 4) & 1, dhw = wi.y >> 6;
                     if (stash && sub < 4) {                                   // lane c files corner c of tap j
-                        const int dw = (wi.y >> 4) & 1, dhw = wi.y >> 5;
                         const int wrow = wi.x + ((sub & 1) ? dw : 0) + ((sub & 2) ? dhw : 0);
                         const int e = ((slot * LP_MAX + k * LPR + j) << 2) + sub;
                         e_row[e] = ((ok >> sub) & 1u) ? (unsigned short)wrow : kNoRow;
@@ -254,10 +289,16 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                     off[1] = off[0] + dwo;
                     off[2] = (unsigned long long)(unsigned)(rr.y & 0x7fffffff) * row_elems;
                     off[3] = off[2] + dwo;
+                    const float4 *srow = vstage + (wi.x - sfirst) * LPR + sub;   // corner 00's staged row (if staged)
 #pragma unroll
                     for (int c = 0; c < 4; ++c) {
                         float v[VEC];
-                        RowVec<float, VEC>::load(base + off[c], v);
+                        if ((sm >> c) & 1u) {
+                            const float4 t = srow[(((c & 1) ? dw : 0) + ((c & 2) ? dhw : 0)) * LPR];
+                            v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+                        } else {
+                            RowVec<float, VEC>::load(base + off[c], v);
+                        }
                         float dsum = 0.f;
 #pragma unroll
                         for (int e = 0; e < VEC; ++e) dsum = fmaf(g[e], v[e], dsum);
