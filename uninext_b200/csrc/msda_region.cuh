@@ -16,11 +16,12 @@
 //   phase A (one 8-lane group per pair, as msda_bwd_tiled): gathers, grad_loc / grad_attn epilogue unchanged; a corner
 //            inside a staged level is read from shared memory, every other corner from global memory (same values, same
 //            FMA order).  The pair's grad_out row is stashed in shared memory; a non-zero corner inside the window
-//            becomes an entry {window row, coefficient} at the fixed position (slot, tap, corner) -- no atomics on the
-//            gather path.  A corner outside the window, or of a query past the stash, reds directly as in
-//            msda_bwd_tiled, so the capacities never change a result.
-//   phase B: counting sort of the entries by window row (integer shared atomics only: fp32 shared atomics are CAS loops)
-//            into {coefficient, slot} arrays, which overlay the staged rows (dead once phase A is done).
+//            becomes an entry {window row, coefficient} at the fixed position (slot, tap, corner), and the filing lane
+//            counts it for its window row with a non-returning shared atomic (nothing on the gather path waits for it).
+//            A corner outside the window, or of a query past the stash, reds directly as in msda_bwd_tiled, so the
+//            capacities never change a result.
+//   phase B: scan of the row counts, then scatter of the entries by window row (integer shared atomics only: fp32 shared
+//            atomics are CAS loops) into {coefficient, slot} arrays, which overlay the staged rows (dead after phase A).
 //   phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
 // A level table that does not tile [0, S) (the patch-order condition) runs in linear chunks of pairs with no window.
 #pragma once
@@ -30,10 +31,10 @@
 namespace msda {
 
 constexpr int kRegionEdge = 8;            // region edge, in pixels of the finest level
-constexpr int kRegionHalo = 4;            // window margin around the scaled region, in pixels of each level
+constexpr int kRegionHalo = 2;            // window margin around the scaled region, in pixels of each level (swept 1-6)
 constexpr int kRegionSlots = 96;          // queries per tile whose grad_out row is stashed (the rest red directly)
 constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past this budget red directly)
-constexpr int kRegionStageRows = 384;     // window rows staged in shared memory (cfg2: levels 1-3, at most 366 rows)
+constexpr int kRegionStageRows = 384;     // window rows staged in shared memory (cfg2: every level, at most 274 rows)
 constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
 constexpr int kRegionMinCtas = 2;
 constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
@@ -45,6 +46,27 @@ constexpr size_t region_smem_bytes() {
     return (size_t)kRegionEntries * (4 + 2) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4 +
            (staged > sorted ? staged : sorted);
 }
+
+#ifdef MSDA_REGION_PHASE_CLOCKS
+// Timing hook for tools/region_phases.py; the library build never defines it.  Thread 0 of each CTA adds the clock64()
+// span since the previous stamp into g_region_clocks[blockIdx.x * 4 + span], after a CTA barrier: span 0 = prologue +
+// tile geometry + staging, 1 = phase A, 2 = phase B, 3 = phase C.  g_region_knockout bit 0 drops phase A's reds, bit 1
+// phase C's (the sums are still formed); results are then wrong by construction and serve only for timing.
+__device__ unsigned long long *g_region_clocks;
+__device__ int g_region_knockout;
+#define MSDA_REGION_CLOCK_INIT long long region_clk = clock64()
+#define MSDA_REGION_CLOCK(span)                                                                  \
+    if (threadIdx.x == 0) {                                                                      \
+        const long long now = clock64();                                                         \
+        g_region_clocks[blockIdx.x * 4 + (span)] += (unsigned long long)(now - region_clk);      \
+        region_clk = now;                                                                        \
+    }
+#define MSDA_REGION_KEEP_RED(bit) (!(g_region_knockout & (bit)))
+#else
+#define MSDA_REGION_CLOCK_INIT
+#define MSDA_REGION_CLOCK(span)
+#define MSDA_REGION_KEEP_RED(bit) true
+#endif
 
 __device__ __forceinline__ void cp_async16(void *dst, const void *src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
@@ -112,6 +134,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
     float *s_coef = reinterpret_cast<float *>(vstage);                                // phases B, C: sorted by window row
     unsigned char *s_slot = reinterpret_cast<unsigned char *>(s_coef + kRegionEntries);
 
+    MSDA_REGION_CLOCK_INIT;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane % LPR, grp = lane / LPR;
     const int LP = L * P;
@@ -192,6 +215,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
         for (int i = threadIdx.x; i < tl.nwin; i += kTiledThreads) cnt[i] = 0;
         cp_async_wait_all();
         __syncthreads();
+        MSDA_REGION_CLOCK(0);
 
         // ---- phase A: gathers, grad_loc / grad_attn; in-window corners become entries, the others red ----
 #pragma unroll 1
@@ -280,8 +304,10 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                     if (stash && sub < 4) {                                   // lane c files corner c of tap j
                         const int wrow = wi.x + ((sub & 1) ? dw : 0) + ((sub & 2) ? dhw : 0);
                         const int e = ((slot * LP_MAX + k * LPR + j) << 2) + sub;
-                        e_row[e] = ((ok >> sub) & 1u) ? (unsigned short)wrow : kNoRow;
+                        const bool filed = (ok >> sub) & 1u;
+                        e_row[e] = filed ? (unsigned short)wrow : kNoRow;
                         e_coef[e] = sub == 0 ? w4.x : sub == 1 ? w4.y : sub == 2 ? w4.z : w4.w;
+                        if (filed) atomicAdd(&cnt[wrow], 1);                  // phase B's row count; result unused
                     }
                     const unsigned dwo = (rr.y < 0) ? row_elems : 0u;
                     unsigned long long off[4];
@@ -303,7 +329,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
 #pragma unroll
                         for (int e = 0; e < VEC; ++e) dsum = fmaf(g[e], v[e], dsum);
                         part[j][c] = dsum;
-                        if (w[c] != 0.f && !((ok >> c) & 1u))
+                        if (w[c] != 0.f && !((ok >> c) & 1u) && MSDA_REGION_KEEP_RED(1))
                             red_add_v4(gbase + off[c], w[c] * g[0], w[c] * g[1], w[c] * g[2], w[c] * g[3]);
                     }
                 }
@@ -321,13 +347,9 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
         const int nwin = tl.nwin;
         if (nwin > 0) {
             __syncthreads();
+            MSDA_REGION_CLOCK(1);
             const int n = min(tl.nq, kRegionSlots) * LP_MAX * 4;
-            // ---- phase B: counting sort of the entries by window row ----
-            for (int e = threadIdx.x; e < n; e += kTiledThreads) {
-                const unsigned short r = e_row[e];
-                if (r != kNoRow) atomicAdd(&cnt[r], 1);
-            }
-            __syncthreads();
+            // ---- phase B: counting sort of the entries by window row (phase A counted them) ----
             {   // exclusive scan of cnt[0, nwin): 4 rows per thread
                 const int i0 = threadIdx.x * 4;
                 int c[4], sum = 0;
@@ -358,6 +380,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                 }
             }
             __syncthreads();          // bucket r is now [r ? cnt[r - 1] : 0, cnt[r]) of s_coef / s_slot
+            MSDA_REGION_CLOCK(2);
 
             // ---- phase C: one group per touched row, one red per lane ----
             const int b = tl.b, m = tl.m;
@@ -376,10 +399,12 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                 while (l + 1 < L && r >= tl.wbase[l + 1]) ++l;
                 const int k = r - tl.wbase[l], y = tl.wy0[l] + k / tl.ww[l], x = tl.wx0[l] + k % tl.ww[l];
                 const int row = rm.start[l] + y * rm.W[l] + x;
-                red_add_v4(grad_value + (((size_t)b * S + row) * M + m) * D + (size_t)sub * VEC, acc.x, acc.y, acc.z, acc.w);
+                if (MSDA_REGION_KEEP_RED(2))
+                    red_add_v4(grad_value + (((size_t)b * S + row) * M + m) * D + (size_t)sub * VEC, acc.x, acc.y, acc.z, acc.w);
             }
         }
         __syncthreads();              // the next tile rewrites tl, the entry list, the stash and the counts
+        MSDA_REGION_CLOCK(nwin > 0 ? 3 : 1);
     }
 }
 
