@@ -32,8 +32,9 @@
  *     grad_out are bfloat16 bit patterns (uint16_t), sampling_loc / attn_weight and their gradients stay fp32,
  *     accumulation is fp32.
  *   - backward: grad_value is zero-filled by the callee (the reference's at::zeros_like, cu:121); grad_sampling_loc
- *     and grad_attn_weight are fully overwritten. grad_value accumulation order is not deterministic (fp32 atomics),
- *     like the reference.
+ *     and grad_attn_weight are fully overwritten.  msda_backward_* accumulate grad_value with atomics, like the
+ *     reference: its summation order, hence its last bits, vary from run to run.  msda_backward_det_* compute the same
+ *     gradients with a fixed summation order (the contract below), at the price of a caller-provided workspace.
  */
 #ifndef MSDA_B200_H_
 #define MSDA_B200_H_
@@ -44,7 +45,7 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 4   /* 4: MSDA_KNOB_REGION_BWD */
+#define MSDA_ABI_VERSION 5   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_* */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -134,6 +135,47 @@ int msda_backward_bf16(const uint16_t *grad_out, const uint16_t *value,
                        int N, int S, int M, int D, int L, int Lq, int P,
                        float *grad_value_f32, uint16_t *grad_value,
                        float *grad_sampling_loc, float *grad_attn_weight, void *stream);
+
+/* ---- deterministic backward (DESIGN.md section 3.10) ----------------------------------------------------------------
+ * Same arguments as msda_backward_* plus a device workspace of `workspace_bytes` bytes (before `stream`).
+ * The contract: grad_value is bit-for-bit what the CPU oracle (oracle/) computes, whatever the launch
+ * geometry, SM count, stream, CUDA graph or chunking:
+ *   - entries: every tap (b, q, m, l, p) passing the window test (h_im > -1 && w_im > -1 && h_im < H && w_im < W)
+ *     contributes, for every corner k inside the map (weight zero included), to row (b, m, r_k);
+ *   - order: within one (b, m, row), contributions are added in ascending e = ((q*M + m)*L*P + l*P + p)*4 + k;
+ *   - rounding: h_im = fl(fl(y*H) - 0.5), lh = h_im - floor(h_im), hh = fl(1 - lh) (w likewise),
+ *     cw = {hh*hw, hh*lw, lh*hw, lh*lw}; contribution fl(cw_k * fl(g_c * a)); acc = fl(acc + contribution) from +0;
+ *     fp64 in double, fp32 and bf16 in float;
+ *   - bf16: grad_out is widened exactly to fp32; the fp32 accumulator `grad_value_f32` follows the rules above and
+ *     `grad_value` (may be NULL) receives its bf16 rounding once.
+ * grad_sampling_loc and grad_attn_weight come from the kernel msda_backward_* would pick at default knob settings, with
+ * its grad_value atomics compiled out: they are bit-identical to msda_backward_*'s.  The knobs are ignored.
+ * grad_value is zero-filled by the callee.  The work runs in chunks of whole queries of one batch element, the largest
+ * that fit the workspace; nothing is allocated, so the call can be captured into a CUDA graph.  Returns MSDA_E_BADARG
+ * if one query does not fit, MSDA_E_TOOLARGE if M*S + 1 > 2^32 or one query's M*L*P*4 entries exceed 2^32 - 1.
+ * msda_backward_det_workspace: bytes needed for chunks of `chunk_queries` queries (>= 1; clipped to Lq); dtype_bytes
+ *   2, 4 or 8.  It asks CUB for the sort's temporary storage, which needs a current CUDA device. */
+int msda_backward_det_workspace(int dtype_bytes, int N, int S, int M, int D, int L, int Lq, int P, int chunk_queries,
+                                int64_t *bytes);
+int msda_backward_det_f32(const float *grad_out, const float *value,
+                          const int64_t *spatial_shapes, const int64_t *level_start_index,
+                          const float *sampling_loc, const float *attn_weight,
+                          int N, int S, int M, int D, int L, int Lq, int P,
+                          float *grad_value, float *grad_sampling_loc, float *grad_attn_weight,
+                          void *workspace, int64_t workspace_bytes, void *stream);
+int msda_backward_det_f64(const double *grad_out, const double *value,
+                          const int64_t *spatial_shapes, const int64_t *level_start_index,
+                          const double *sampling_loc, const double *attn_weight,
+                          int N, int S, int M, int D, int L, int Lq, int P,
+                          double *grad_value, double *grad_sampling_loc, double *grad_attn_weight,
+                          void *workspace, int64_t workspace_bytes, void *stream);
+int msda_backward_det_bf16(const uint16_t *grad_out, const uint16_t *value,
+                           const int64_t *spatial_shapes, const int64_t *level_start_index,
+                           const float *sampling_loc, const float *attn_weight,
+                           int N, int S, int M, int D, int L, int Lq, int P,
+                           float *grad_value_f32, uint16_t *grad_value,
+                           float *grad_sampling_loc, float *grad_attn_weight,
+                           void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---- callers of the op (SURVEY.md section 8 rows f-1 / f-2): one-pass fp32 kernels around the cuBLAS GEMMs --------
  * msda_prologue_forward_f32: raw projection -> attention softmax + sampling locations in the op's layouts.

@@ -28,6 +28,10 @@ SIGNATURES = {
     "msda_backward_f32": (_i, [_vp] * 6 + _DIMS + [_vp] * 3 + [_vp]),
     "msda_backward_f64": (_i, [_vp] * 6 + _DIMS + [_vp] * 3 + [_vp]),
     "msda_backward_bf16": (_i, [_vp] * 6 + _DIMS + [_vp] * 4 + [_vp]),
+    "msda_backward_det_workspace": (_i, [_i] * 9 + [_vp]),
+    "msda_backward_det_f32": (_i, [_vp] * 6 + _DIMS + [_vp] * 3 + [_vp, ctypes.c_int64, _vp]),
+    "msda_backward_det_f64": (_i, [_vp] * 6 + _DIMS + [_vp] * 3 + [_vp, ctypes.c_int64, _vp]),
+    "msda_backward_det_bf16": (_i, [_vp] * 6 + _DIMS + [_vp] * 4 + [_vp, ctypes.c_int64, _vp]),
     "msda_prologue_forward_f32": (_i, [_vp] * 3 + [ctypes.c_int64, _i, _i, _i, _i] + [_vp] * 3),
     "msda_prologue_backward_f32": (_i, [_vp] * 5 + [ctypes.c_int64, _i, _i, _i, _i] + [_vp] * 2),
     "msda_colsum_f32": (_i, [_vp, ctypes.c_int64, _i, _vp, _vp]),
@@ -47,7 +51,7 @@ SIGNATURES = {
     "msda_aligned_bilinear_forward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
     "msda_aligned_bilinear_backward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
 }
-ABI_VERSION = 4
+ABI_VERSION = 5
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 

@@ -7,6 +7,7 @@
 
 #include "../../include/msda_b200.h"
 #include "msda_condinst.cuh"
+#include "msda_det.cuh"
 #include "msda_generic.cuh"
 #include "msda_module.cuh"
 #include "msda_region.cuh"
@@ -232,7 +233,7 @@ cudaError_t launch_after_fill(K kern, int grid, size_t smem, cudaStream_t st, Ar
     return cudaGetLastError();
 }
 
-template <typename T, int D, int LP_MAX, int VEC = BwdVec<T>::v>
+template <typename T, int D, int LP_MAX, int VEC = BwdVec<T>::v, bool NORED = false>
 cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
                        const float *attn, const Dims &d, float *gv, float *gl, float *ga, cudaStream_t st) {
     constexpr int GPW = 32 / (D / VEC);
@@ -241,13 +242,13 @@ cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes,
     const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
     const bool split = kCanSplit && use_split(npairs);
     const bool tma = !split && kCanStage && use_tma_staging(d);
-    auto kern = split ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit>
-                : tma ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false>
-                      : msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false>;
+    auto kern = split ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit, false, NORED>
+                : tma ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false, false, NORED>
+                      : msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>;
     static std::atomic<int> c_split[kMaxDevices], c_tma[kMaxDevices], c_ldg[kMaxDevices];
-    const int slots = split ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit>, c_split)
-                      : tma ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false>, c_tma)
-                            : resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false>, c_ldg);
+    const int slots = split ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit, false, NORED>, c_split)
+                      : tma ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false, false, NORED>, c_tma)
+                            : resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>, c_ldg);
     const unsigned iter_pairs = msda::kTiledWarps * (split ? 1 : GPW);
     const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;
     const int grid = (int)(tiles_ub < (unsigned)slots ? tiles_ub : (unsigned)slots);
@@ -470,7 +471,7 @@ cudaError_t fwd_generic(const T *value, const int64_t *shapes, const int64_t *ls
     return cudaGetLastError();
 }
 
-template <typename T, typename TL, typename GA>
+template <typename T, typename TL, typename GA, bool NORED = false>
 cudaError_t bwd_generic(const T *go, const T *value, const int64_t *shapes, const int64_t *lsi, const TL *loc,
                         const TL *attn, const Dims &d, GA *gv, TL *gl, TL *ga, cudaStream_t st) {
     const long long npairs = (long long)d.N * d.Lq * d.M;
@@ -479,10 +480,144 @@ cudaError_t bwd_generic(const T *go, const T *value, const int64_t *shapes, cons
     long long blocks = npairs;
     const long long cap = (long long)num_sms() * 64;
     if (blocks > cap) blocks = cap;
-    msda::msda_bwd_generic<T, TL, GA><<<(int)blocks, threads, 0, st>>>(go, value, shapes, lsi, loc, attn, d.S, d.M, d.D,
-                                                                       d.L, d.Lq, d.P, npairs, gv, gl, ga);
+    msda::msda_bwd_generic<T, TL, GA, NORED><<<(int)blocks, threads, 0, st>>>(go, value, shapes, lsi, loc, attn, d.S, d.M,
+                                                                              d.D, d.L, d.Lq, d.P, npairs, gv, gl, ga);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
+}
+
+
+// ---- deterministic backward (msda_det.cuh) ------------------------------------------------------------------------
+// Workspace of one chunk of nq queries (n = nq*M*L*P*4 entries): sort keys and values in and out (4 x n x 4 bytes), the
+// segment starts (M*S + 1 words), the row counter of the accumulate step and CUB's temporary storage, each 256-byte aligned.
+struct DetLayout { size_t keys_in, keys_out, vals_in, vals_out, start, counter, temp, temp_bytes, total; unsigned n; };
+
+int det_end_bit(const Dims &d) {                   // bits of the largest key, the sentinel M*S
+    const unsigned long long top = (unsigned long long)d.M * d.S;
+    int bits = 0;
+    while (bits < 32 && (top >> bits) != 0) ++bits;
+    return bits;
+}
+
+int det_layout(const Dims &d, long long nq, DetLayout &lay) {
+    const unsigned long long n = (unsigned long long)nq * d.M * d.L * d.P * 4;
+    if (n > 0xffffffffull) return MSDA_E_TOOLARGE;
+    lay.n = (unsigned)n;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) & ~(size_t)255; return at; };
+    lay.keys_in = take(4 * n);
+    lay.keys_out = take(4 * n);
+    lay.vals_in = take(4 * n);
+    lay.vals_out = take(4 * n);
+    lay.start = take(4 * ((size_t)d.M * d.S + 1));
+    lay.counter = take(4);
+    lay.temp_bytes = 0;
+    const cudaError_t e = msda::det_sort(nullptr, lay.temp_bytes, nullptr, nullptr, nullptr, nullptr, lay.n, det_end_bit(d), 0);
+    if (e != cudaSuccess) return (int)e;
+    lay.temp = take(lay.temp_bytes);
+    lay.total = off;
+    return 0;
+}
+
+int det_check(const Dims &d) {
+    if (int e = check_dims(d)) return e;
+    if ((unsigned long long)d.M * d.S + 1 > (1ull << 32)) return MSDA_E_TOOLARGE;     // keys and the sentinel are 32-bit
+    return 0;
+}
+
+// grad_loc / grad_attn: the kernel the default route picks (the region kernel's are bit-identical to msda_bwd_tiled's),
+// with its grad_value reds compiled out.
+template <typename T, typename TL, typename GA>
+cudaError_t det_loc_attn(const T *go, const T *value, const int64_t *shapes, const int64_t *lsi, const TL *loc,
+                         const TL *attn, const Dims &d, bool fast, GA *gv, TL *gl, TL *ga, cudaStream_t st) {
+    if constexpr (sizeof(T) != 8) {
+        if (fast) {
+            const int LP = d.L * d.P;
+            switch (d.D) {
+                case 16:
+                    if constexpr (sizeof(T) == 4)
+                        return LP <= 16 ? launch_bwd<T, 16, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
+                                        : launch_bwd<T, 16, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+                    break;
+                case 32:
+                    return LP <= 16 ? launch_bwd<T, 32, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
+                                    : launch_bwd<T, 32, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+                case 64:
+                    return LP <= 16 ? launch_bwd<T, 64, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
+                                    : launch_bwd<T, 64, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+            }
+            return cudaErrorInvalidValue;
+        }
+    }
+    return bwd_generic<T, TL, GA, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+}
+
+// The whole deterministic backward into the zero-filled accumulator gv (compute type of T).  `fast`: the default route
+// would take the tiled kernels (16-byte aligned tensors, fast-path shape).
+template <typename T, typename TL>
+int det_backward(const T *go, const T *value, const int64_t *shapes, const int64_t *lsi, const TL *loc, const TL *attn,
+                 const Dims &d, bool fast, typename msda::Num<T>::C *gv, TL *gl, TL *ga, void *ws, int64_t ws_bytes,
+                 cudaStream_t st) {
+    using C = typename msda::Num<T>::C;
+    if (ws == nullptr || ws_bytes <= 0) return MSDA_E_BADARG;
+    DetLayout lay{};
+    if (int e = det_layout(d, 1, lay)) return e;
+    if ((long long)lay.total > ws_bytes) return MSDA_E_BADARG;           // one query does not fit
+    long long lo = 1, hi = d.Lq;                                         // largest chunk that fits
+    while (lo < hi) {
+        const long long mid = hi - (hi - lo) / 2;
+        DetLayout t{};
+        const int e = det_layout(d, mid, t);
+        if (e == 0 && (long long)t.total <= ws_bytes) lo = mid; else if (e != 0 && e != MSDA_E_TOOLARGE) return e; else hi = mid - 1;
+    }
+    const long long chunk = lo;
+    cudaError_t err = cudaMemsetAsync(gv, 0, sizeof(C) * (size_t)d.N * d.S * d.M * d.D, st);
+    if (err != cudaSuccess) return (int)err;
+    err = det_loc_attn<T, TL, C>(go, value, shapes, lsi, loc, attn, d, fast, gv, gl, ga, st);
+    if (err != cudaSuccess) return (int)err;
+
+    unsigned char *w = static_cast<unsigned char *>(ws);
+    const int end_bit = det_end_bit(d);
+    const unsigned nkeys = (unsigned)d.M * (unsigned)d.S;
+    const bool v4 = sizeof(T) != 8 && d.D == 32 && fast;
+    const int sms = num_sms();
+    const int LP = d.L * d.P;
+    for (int b = 0; b < d.N; ++b) {
+        for (long long q0 = 0; q0 < d.Lq; q0 += chunk) {
+            const long long nq = q0 + chunk <= d.Lq ? chunk : d.Lq - q0;
+            if (int e = det_layout(d, nq, lay)) return e;
+            unsigned *keys_in = reinterpret_cast<unsigned *>(w + lay.keys_in), *keys_out = reinterpret_cast<unsigned *>(w + lay.keys_out);
+            unsigned *vals_in = reinterpret_cast<unsigned *>(w + lay.vals_in), *vals_out = reinterpret_cast<unsigned *>(w + lay.vals_out);
+            unsigned *start = reinterpret_cast<unsigned *>(w + lay.start), *counter = reinterpret_cast<unsigned *>(w + lay.counter);
+            const long long tap0 = ((long long)b * d.Lq + q0) * d.M * LP;
+            const T *go_chunk = go + ((size_t)b * d.Lq + q0) * d.M * d.D;
+            long long blocks = ((long long)lay.n + msda::kDetThreads - 1) / msda::kDetThreads;
+            if (blocks > (long long)sms * 16) blocks = (long long)sms * 16;
+            msda::msda_det_keys<TL><<<(int)blocks, msda::kDetThreads, 0, st>>>(loc, shapes, lsi, d.S, d.M, d.L, d.P, tap0,
+                                                                               lay.n, keys_in, vals_in);
+            if ((err = cudaGetLastError()) != cudaSuccess) return (int)err;
+            size_t temp_bytes = lay.temp_bytes;
+            err = msda::det_sort(w + lay.temp, temp_bytes, keys_in, keys_out, vals_in, vals_out, lay.n, end_bit, st);
+            if (err != cudaSuccess) return (int)err;
+            long long kblocks = ((long long)nkeys + 1 + msda::kDetThreads - 1) / msda::kDetThreads;
+            if (kblocks > (long long)sms * 16) kblocks = (long long)sms * 16;
+            msda::msda_det_bounds<<<(int)kblocks, msda::kDetThreads, 0, st>>>(keys_out, lay.n, nkeys, start);
+            if ((err = cudaGetLastError()) != cudaSuccess) return (int)err;
+            if ((err = cudaMemsetAsync(counter, 0, 4, st)) != cudaSuccess) return (int)err;
+            if constexpr (sizeof(T) != 8) {
+                if (v4) {
+                    msda::msda_det_accumulate_v4<T><<<sms * 8, msda::kDetThreads, 0, st>>>(
+                        go_chunk, loc, attn, shapes, d.S, d.M, d.L, d.P, tap0, b, start, vals_out, counter, gv);
+                }
+            }
+            if (!v4)
+                msda::msda_det_accumulate<T, TL><<<sms * 8, msda::kDetThreads, 0, st>>>(
+                    go_chunk, loc, attn, shapes, d.S, d.M, d.D, d.L, d.P, tap0, b, start, vals_out, counter, gv);
+            if ((err = cudaGetLastError()) != cudaSuccess) return (int)err;
+            g_launches.fetch_add(4, std::memory_order_relaxed);       // keys, sort (counted once), bounds, accumulate
+        }
+    }
+    return 0;
 }
 
 }  // namespace
@@ -656,6 +791,71 @@ int msda_backward_bf16(const uint16_t *grad_out, const uint16_t *value, const in
         err = cudaGetLastError();
     }
     return (int)err;
+}
+
+
+int msda_backward_det_workspace(int dtype_bytes, int N, int S, int M, int D, int L, int Lq, int P, int chunk_queries,
+                                int64_t *bytes) {
+    const Dims d{N, S, M, D, L, Lq, P};
+    if (dtype_bytes != 2 && dtype_bytes != 4 && dtype_bytes != 8) return MSDA_E_BADARG;
+    if (!bytes || chunk_queries <= 0) return MSDA_E_BADARG;
+    if (int e = det_check(d)) return e;
+    DetLayout lay{};
+    if (int e = det_layout(d, chunk_queries < Lq ? chunk_queries : Lq, lay)) return e;
+    *bytes = (int64_t)lay.total;
+    return 0;
+}
+
+int msda_backward_det_f32(const float *grad_out, const float *value, const int64_t *spatial_shapes,
+                          const int64_t *level_start_index, const float *sampling_loc, const float *attn_weight, int N,
+                          int S, int M, int D, int L, int Lq, int P, float *grad_value, float *grad_sampling_loc,
+                          float *grad_attn_weight, void *workspace, int64_t workspace_bytes, void *stream) {
+    const Dims d{N, S, M, D, L, Lq, P};
+    if (int e = det_check(d)) return e;
+    MSDA_CHECK_PTRS(al, grad_out, value, sampling_loc, attn_weight, grad_value, grad_sampling_loc, grad_attn_weight);
+    if (!spatial_shapes || !level_start_index) return MSDA_E_BADARG;
+    return det_backward<float, float>(grad_out, value, spatial_shapes, level_start_index, sampling_loc, attn_weight, d,
+                                      al && use_fast(4, d), grad_value, grad_sampling_loc, grad_attn_weight, workspace,
+                                      workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int msda_backward_det_f64(const double *grad_out, const double *value, const int64_t *spatial_shapes,
+                          const int64_t *level_start_index, const double *sampling_loc, const double *attn_weight, int N,
+                          int S, int M, int D, int L, int Lq, int P, double *grad_value, double *grad_sampling_loc,
+                          double *grad_attn_weight, void *workspace, int64_t workspace_bytes, void *stream) {
+    const Dims d{N, S, M, D, L, Lq, P};
+    if (int e = det_check(d)) return e;
+    if (!grad_out || !value || !spatial_shapes || !level_start_index || !sampling_loc || !attn_weight || !grad_value ||
+        !grad_sampling_loc || !grad_attn_weight)
+        return MSDA_E_BADARG;
+    return det_backward<double, double>(grad_out, value, spatial_shapes, level_start_index, sampling_loc, attn_weight, d,
+                                        false, grad_value, grad_sampling_loc, grad_attn_weight, workspace, workspace_bytes,
+                                        static_cast<cudaStream_t>(stream));
+}
+
+int msda_backward_det_bf16(const uint16_t *grad_out, const uint16_t *value, const int64_t *spatial_shapes,
+                           const int64_t *level_start_index, const float *sampling_loc, const float *attn_weight, int N,
+                           int S, int M, int D, int L, int Lq, int P, float *grad_value_f32, uint16_t *grad_value,
+                           float *grad_sampling_loc, float *grad_attn_weight, void *workspace, int64_t workspace_bytes,
+                           void *stream) {
+    const Dims d{N, S, M, D, L, Lq, P};
+    if (int e = det_check(d)) return e;
+    MSDA_CHECK_PTRS(al, grad_out, value, sampling_loc, attn_weight, grad_value_f32, grad_sampling_loc, grad_attn_weight);
+    if (!spatial_shapes || !level_start_index) return MSDA_E_BADARG;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int e = det_backward<__nv_bfloat16, float>(
+        reinterpret_cast<const __nv_bfloat16 *>(grad_out), reinterpret_cast<const __nv_bfloat16 *>(value), spatial_shapes,
+        level_start_index, sampling_loc, attn_weight, d, al && use_fast(2, d), grad_value_f32, grad_sampling_loc,
+        grad_attn_weight, workspace, workspace_bytes, st);
+    if (e != 0 || grad_value == nullptr) return e;
+    const size_t nval = (size_t)N * S * M * D;
+    long long blocks = (long long)((nval + 255) / 256);
+    const long long cap = (long long)num_sms() * 16;
+    if (blocks > cap) blocks = cap;
+    msda::msda_f32_to_bf16<<<(int)blocks, 256, 0, st>>>(grad_value_f32, reinterpret_cast<__nv_bfloat16 *>(grad_value),
+                                                        (long long)nval);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)cudaGetLastError();
 }
 
 

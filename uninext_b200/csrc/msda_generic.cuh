@@ -93,8 +93,8 @@ __device__ __forceinline__ C block_sum(C v, C *scratch) {
 }
 
 // One block per (b,q,m) pair, threads stride over channels.  GA is the grad_value accumulator type
-// (T for fp32/fp64, float for bf16 storage).
-template <typename T, typename TL, typename GA>
+// (T for fp32/fp64, float for bf16 storage).  NORED: grad_loc / grad_attn only (the deterministic backward, msda_det.cuh).
+template <typename T, typename TL, typename GA, bool NORED = false>
 __global__ void __launch_bounds__(256)
 msda_bwd_generic(const T *__restrict__ grad_out, const T *__restrict__ value,
                  const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
@@ -129,7 +129,7 @@ msda_bwd_generic(const T *__restrict__ grad_out, const T *__restrict__ value,
                             if (g.r[k] >= 0) {
                                 const size_t o = slab + (size_t)g.r[k] * row_elems + c;
                                 v[k] = Num<T>::ld(value + o);
-                                atomicAdd(grad_value + o, (GA)(cw[k] * a * go));            // cuh:125,134,143,152
+                                if constexpr (!NORED) atomicAdd(grad_value + o, (GA)(cw[k] * a * go));   // cuh:125,134,143,152
                             }
                         }
                         ga += go * (cw[0] * v[0] + cw[1] * v[1] + cw[2] * v[2] + cw[3] * v[3]);     // cuh:156

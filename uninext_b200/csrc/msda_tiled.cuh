@@ -404,7 +404,8 @@ __device__ __forceinline__ void finish_tap(const float (&dot)[4], unsigned mk, f
 // bytes through the SM's crossbar port, which is what bounds this kernel -- while the coarse levels (hundreds to
 // thousands of contributions per row) keep the fp32 accumulator.  The fine flag travels in bit 31 of the record's row
 // index (rows are < 2^30).
-template <typename T, int VEC, int D, int LP_MAX, int MIN_CTAS, bool TMA, bool SPLIT, bool MIXED = false>
+// NORED: grad_loc / grad_attn only, grad_value untouched (the deterministic backward sums grad_value itself, msda_det.cuh).
+template <typename T, int VEC, int D, int LP_MAX, int MIN_CTAS, bool TMA, bool SPLIT, bool MIXED = false, bool NORED = false>
 __global__ void __launch_bounds__(kTiledThreads, MIN_CTAS)
 msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
                const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
@@ -414,6 +415,7 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
                __nv_bfloat16 *__restrict__ grad_value_bf16, int fine_min_rows)
 {
     static_assert(!MIXED || (sizeof(T) == 2 && VEC == 4), "MIXED accumulates bf16 rows with 8-byte packed reds");
+    static_assert(!(MIXED && NORED), "MIXED accumulates grad_value");
     constexpr int LPR = D / VEC;
     constexpr int GPW = 32 / LPR;
     constexpr int PPW = SPLIT ? 1 : GPW;                    // see msda_fwd_tiled
@@ -546,11 +548,13 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
                             const bool nz = w[c] != 0.f;
                             red_add_mixed(nz && fine, grad_value_bf16 + slab_off + off[c], nz && !fine, gbase + off[c],
                                           w[c] * g[0], w[c] * g[1], w[c] * g[2], w[c] * g[3]);
-                        } else if (w[c] != 0.f) {     // masked-out corners, dead taps and idle groups carry weight 0
+                        } else if constexpr (!NORED) {
+                            if (w[c] != 0.f) {        // masked-out corners, dead taps and idle groups carry weight 0
 #pragma unroll
-                            for (int e = 0; e < VEC; e += 4)
-                                red_add_v4(gbase + off[c] + e, w[c] * g[e], w[c] * g[e + 1], w[c] * g[e + 2],
-                                           w[c] * g[e + 3]);
+                                for (int e = 0; e < VEC; e += 4)
+                                    red_add_v4(gbase + off[c] + e, w[c] * g[e], w[c] * g[e + 1], w[c] * g[e + 2],
+                                               w[c] * g[e + 3]);
+                            }
                         }
                     }
                 }

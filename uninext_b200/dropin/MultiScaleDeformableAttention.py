@@ -7,17 +7,26 @@ The reference builds a pybind11 extension with this name (ops/setup.py:53, ops/s
 
 Exports exactly the reference's two functions with the reference's signatures, checks and error type
 (``RuntimeError``; ops/src/ms_deform_attn.h:19-62, ops/src/cuda/ms_deform_attn_cuda.cu:28-52,93-116).
-Beyond the reference: bfloat16 ``value`` is accepted (sampling locations / attention weights are then taken as fp32).
+Beyond the reference: bfloat16 ``value`` is accepted (sampling locations / attention weights are then taken as fp32),
+and under ``torch.use_deterministic_algorithms(True)`` the backward sums grad_value in a fixed order
+(msda_backward_det_*, include/msda_b200.h), bit-for-bit reproducible from run to run.
 """
 from __future__ import annotations
+
+import ctypes
 
 import torch
 
 from uninext_b200 import _cabi
+from uninext_b200._determinism import deterministic_requested
 
 __all__ = ["ms_deform_attn_forward", "ms_deform_attn_backward"]
 
 _SUFFIX = {torch.float32: "f32", torch.float64: "f64", torch.bfloat16: "bf16"}
+
+# Upper bound of the deterministic backward's workspace (torch's caching allocator).  Calls that need more run in
+# chunks of queries; a cfg2 encoder batch element needs ~11.4 M entries x 16 B ~ 183 MB plus the sort's temporary storage.
+DET_WORKSPACE_CAP = 256 << 20
 
 
 def _checks(named, value, im2col_step):
@@ -102,11 +111,28 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
     return out
 
 
+def _det_workspace(lib, value, dims):
+    """Workspace of msda_backward_det_*: the whole call in one pass when it fits DET_WORKSPACE_CAP, otherwise the cap
+    (the library then runs the largest query chunks that fit), and at least one query's worth."""
+    lq = dims[5]
+    need, one = ctypes.c_int64(0), ctypes.c_int64(0)
+    _cabi.check(lib.msda_backward_det_workspace(value.element_size(), *dims, lq, ctypes.byref(need)),
+                "msda_backward_det_workspace")
+    nbytes = need.value
+    if nbytes > DET_WORKSPACE_CAP:
+        _cabi.check(lib.msda_backward_det_workspace(value.element_size(), *dims, 1, ctypes.byref(one)),
+                    "msda_backward_det_workspace")
+        nbytes = max(DET_WORKSPACE_CAP, one.value)
+    return torch.empty(nbytes, dtype=torch.uint8, device=value.device)
+
+
 def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
-                            im2col_step, grad_value_dtype=None):
+                            im2col_step, grad_value_dtype=None, deterministic=None):
     """-> [grad_value, grad_sampling_loc, grad_attn_weight]   (reference ms_deform_attn_cuda_backward, cu:83-153).
     ``grad_value_dtype=torch.float32`` (bf16 ``value`` only, beyond the reference): hand back the fp32 accumulator
-    itself instead of its bf16 rounding -- no conversion pass, no second buffer."""
+    itself instead of its bf16 rounding -- no conversion pass, no second buffer.
+    ``deterministic`` (beyond the reference): True sums grad_value in the fixed order of msda_backward_det_*; None follows
+    ``torch.are_deterministic_algorithms_enabled()``.  grad_sampling_loc / grad_attn_weight are the same either way."""
     _checks([("value", value), ("spatial_shapes", spatial_shapes), ("level_start_index", level_start_index),
              ("sampling_loc", sampling_loc), ("attn_weight", attn_weight), ("grad_output", grad_output)],
             value, im2col_step)
@@ -121,21 +147,25 @@ def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_l
         return [torch.zeros(value.shape, dtype=gv_dtype, device=value.device), torch.zeros_like(sampling_loc),
                 torch.zeros_like(attn_weight)]
     lib = _cabi.load()
+    det = deterministic_requested() if deterministic is None else bool(deterministic)
     with torch.cuda.device(value.device):
         grad_loc = torch.empty_like(sampling_loc)
         grad_attn = torch.empty_like(attn_weight)
         stream = torch.cuda.current_stream().cuda_stream
         common = (grad_output.data_ptr(), value.data_ptr(), spatial_shapes.data_ptr(), level_start_index.data_ptr(),
                   sampling_loc.data_ptr(), attn_weight.data_ptr(), *dims)
+        ws = _det_workspace(lib, value, dims) if det else None
+        tail = (ws.data_ptr(), ws.numel(), stream) if det else (stream,)
+        kind = "msda_backward_det_" if det else "msda_backward_"
         if value.dtype == torch.bfloat16:
             acc = torch.empty(value.shape, dtype=torch.float32, device=value.device)
             keep_f32 = grad_value_dtype == torch.float32
             grad_value = acc if keep_f32 else torch.empty_like(value)
-            code = lib.msda_backward_bf16(*common, acc.data_ptr(), None if keep_f32 else grad_value.data_ptr(),
-                                          grad_loc.data_ptr(), grad_attn.data_ptr(), stream)
+            code = getattr(lib, kind + "bf16")(*common, acc.data_ptr(), None if keep_f32 else grad_value.data_ptr(),
+                                               grad_loc.data_ptr(), grad_attn.data_ptr(), *tail)
         else:
-            grad_value = torch.empty_like(value)          # zero-filled by the callee (cudaMemsetAsync on `stream`)
-            fn = getattr(lib, "msda_backward_" + _SUFFIX[value.dtype])
-            code = fn(*common, grad_value.data_ptr(), grad_loc.data_ptr(), grad_attn.data_ptr(), stream)
+            grad_value = torch.empty_like(value)          # zero-filled by the callee on `stream`
+            fn = getattr(lib, kind + _SUFFIX[value.dtype])
+            code = fn(*common, grad_value.data_ptr(), grad_loc.data_ptr(), grad_attn.data_ptr(), *tail)
     _cabi.check(code, "ms_deform_attn_backward")
     return [grad_value, grad_loc, grad_attn]

@@ -10,7 +10,8 @@ single hand-written kernels.
 * ``add_layer_norm``      -- ``LayerNorm(a + b)`` (deformable_transformer.py:354-356,359) forward and backward.
 
 These wrappers are conveniences for the callers of the op: when their preconditions do not hold (non-fp32, CPU tensors,
-unsupported widths) they hand the same maths to the stock torch ops.  The op itself (MSDeformAttnFunction) has no such
+unsupported widths, or ``torch.use_deterministic_algorithms(True)``: the column sums of the bias / LayerNorm gradients use
+float atomics) they hand the same maths to the stock torch ops.  The op itself (MSDeformAttnFunction) has no such
 path: it raises without the CUDA library.
 """
 from __future__ import annotations
@@ -20,6 +21,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from uninext_b200 import _cabi
+from uninext_b200._determinism import deterministic_requested
 
 
 def _stream():
@@ -33,7 +35,7 @@ def _f32c(t):
 def colsum(x2d: torch.Tensor) -> torch.Tensor:
     """sum over rows of a contiguous fp32 [rows, cols] CUDA tensor (cols % 4 == 0)."""
     rows, cols = x2d.shape
-    if cols % 4 or x2d.data_ptr() % 16:
+    if cols % 4 or x2d.data_ptr() % 16 or deterministic_requested():
         return x2d.sum(0)
     out = torch.empty(cols, dtype=torch.float32, device=x2d.device)
     with torch.cuda.device(x2d.device):
@@ -150,7 +152,8 @@ class _LinearColsum(Function):
         x2, weight, y, mask = ctx.saved_tensors
         g2 = g.reshape(-1, g.shape[-1])
         gb = None
-        if ctx.relu and g2.is_cuda and g2.dtype == torch.float32 and g2.shape[1] % 4 == 0 and ctx.needs_input_grad[2]:
+        if ctx.relu and g2.is_cuda and g2.dtype == torch.float32 and g2.shape[1] % 4 == 0 and ctx.needs_input_grad[2] \
+                and not deterministic_requested():
             # ReLU backward and the bias gradient in ONE pass over (g, y)  (masked rows have y == 0: zeroed by the same test)
             g2 = g2.contiguous()
             out = torch.empty_like(g2)
@@ -323,7 +326,8 @@ def add_layer_norm(a, b, norm: torch.nn.LayerNorm):
     auto = torch.is_autocast_enabled()               # under autocast the inputs are cast to fp32 by custom_fwd
     ok = a.is_cuda and (a.dtype == torch.float32 or auto) and cols in (128, 256, 384, 512) and norm.elementwise_affine \
         and norm.bias is not None and (b is None or b.dtype == torch.float32 or auto) \
-        and all(t is None or t.data_ptr() % 16 == 0 for t in (a, b, norm.weight, norm.bias))      # float4 loads in the kernels
+        and all(t is None or t.data_ptr() % 16 == 0 for t in (a, b, norm.weight, norm.bias)) \
+        and not deterministic_requested()                          # dgamma / dbeta are summed with float atomics
     if not ok:
         return norm(a if b is None else a + b)
     return _AddLayerNorm.apply(a, b, norm.weight, norm.bias, norm.eps)

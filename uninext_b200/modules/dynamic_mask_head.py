@@ -22,6 +22,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from uninext_b200 import _cabi
+from uninext_b200._determinism import alert_not_deterministic
 
 from .deformable_transformer import MLP
 
@@ -105,6 +106,7 @@ class _DynamicMaskHead(Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
+        alert_not_deterministic("_DynamicMaskHead.backward (msda_condinst_backward_f32 sums with float atomics)")
         lib = _cabi.load()
         feats, params, refs, inst_start = ctx.saved_tensors
         stride, rel, max_inst = ctx.cfg
