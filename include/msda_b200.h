@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 5   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_* */
+#define MSDA_ABI_VERSION 6   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_* */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -258,6 +258,36 @@ int msda_linear_tf32(const float *A, const float *W, const float *bias, int64_t 
 int msda_linear_tf32_ex(const float *A, const float *W, const float *bias, const uint8_t *row_mask, int64_t M, int N, int K,
                         int relu, float *C, void *stream);
 int msda_linear_tf32_ws_ok(int N, int K);
+
+/* ---- fused image-text attention of the early-fusion block (DESIGN.md section 3.11; fuse_helper.py:54-139) ----------
+ * Per (b, h): x = clamp(Q K^T) (clamp_min / clamp_max: the clamps at -50000 / 50000), P_v = softmax over T of
+ * (x + text_bias[b]), P_l = softmax over S of (x^T - max over S of x^T), O_v = dropout(P_v) Vl, O_l = dropout(P_l) Vv.
+ *   q, v_v, out_v      [B, S, H, head_dim]   (q already multiplied by head_dim^-0.5)
+ *   k, v_l, out_l      [B, T, H, head_dim]
+ *   text_bias          [B, T] fp32 additive mask, as the reference adds it (-9e15 at padding), or NULL
+ *   stats              [B*H*(S + T)*2] fp32: per-row and per-column softmax statistics saved for the backward
+ *   seed               device int64 scalar keying the dropout masks (counter-based Philox); read only when
+ *                      dropout_p > 0.  The same seed gives the same masks in the forward, the backward and
+ *                      msda_vlfuse_dropout_mask_f32.
+ * Limits: head_dim 128 or 256, 1 <= T <= 256, 0 <= dropout_p < 1; every tensor pointer 16-byte aligned and contiguous.
+ * No S x T tensor is stored and no float atomics are used: every output is bit-identical from run to run.  Nothing is
+ * allocated and nothing synchronises with the host; the calls can be captured into a CUDA graph.
+ * msda_vlfuse_workspace: bytes of `workspace` both calls need for these sizes.
+ * msda_vlfuse_backward_f32 writes all four gradients (overwritten, not accumulated).
+ * msda_vlfuse_dropout_mask_f32: the keep decisions as 1.0 / 0.0, mask_v [B*H, S, T] (vision), mask_l [B*H, T, S] (text). */
+int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *bytes);
+int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
+                            int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
+                            const int64_t *seed, float *out_v, float *out_l, float *stats, void *workspace,
+                            int64_t workspace_bytes, void *stream);
+int msda_vlfuse_backward_f32(const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
+                             const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
+                             const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
+                             int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
+                             float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
+                             void *stream);
+int msda_vlfuse_dropout_mask_f32(const int64_t *seed, int B, int H, int S, int T, float dropout_p, float *mask_v,
+                                 float *mask_l, void *stream);
 
 #ifdef __cplusplus
 }

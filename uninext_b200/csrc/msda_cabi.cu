@@ -14,6 +14,7 @@
 #include "msda_slab.cuh"
 #include "msda_tmem.cuh"
 #include "msda_tiled.cuh"
+#include "msda_vlfuse.cuh"
 
 namespace {
 
@@ -1106,6 +1107,165 @@ int msda_sine_pos_embed_backward_f32(const float *pos, const float *grad_out, in
     const long long warps = (long long)R * n;
     msda::msda_sine_pos_embed<true><<<(unsigned)((warps * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         pos, grad_out, R, n, F, temperature, exchange_xy, grad_pos);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)cudaGetLastError();
+}
+
+}  // extern "C"
+
+// ---- fused image-text attention of the early-fusion block (msda_vlfuse.cuh) -----------------------------------------
+namespace {
+
+struct VlfLayout {
+    size_t part0, part1, colpart, delta_v, delta_l, total;
+    int row_tiles, col_tiles, nsplit, split_rows;
+};
+
+inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
+
+// Workspace carve-up.  The image-token ranges of the column-side kernels depend on the shape only (about 1024 CTAs), so
+// the summation order, hence every bit of the result, does not depend on the device.
+VlfLayout vlf_layout(int B, int H, int S, int T, int D) {
+    VlfLayout l{};
+    const long long BH = (long long)B * H;
+    l.row_tiles = (S + vlf::kRowTile - 1) / vlf::kRowTile;
+    l.col_tiles = (T + vlf::kColTile - 1) / vlf::kColTile;
+    const long long per = BH * l.col_tiles, want = (1024 + per - 1) / per;
+    long long rows = (S + want - 1) / want;
+    rows = (rows + vlf::kChunkS - 1) / vlf::kChunkS * vlf::kChunkS;
+    l.split_rows = (int)rows;
+    l.nsplit = (int)((S + rows - 1) / rows);
+    const size_t part = align256(sizeof(float) * (size_t)l.nsplit * BH * T * D);
+    l.part0 = 0;
+    l.part1 = l.colpart = part;                                             // forward: part0 + colpart
+    const size_t fwd = part + align256(sizeof(float) * (size_t)BH * l.row_tiles * T * 2);
+    l.delta_v = 2 * part;                                                   // backward: part0 + part1 + deltas
+    l.delta_l = l.delta_v + align256(sizeof(float) * (size_t)BH * S);
+    const size_t bwd = l.delta_l + align256(sizeof(float) * (size_t)BH * T);
+    l.total = fwd > bwd ? fwd : bwd;
+    return l;
+}
+
+int vlf_check(int B, int H, int S, int T, int D, float p) {
+    if (B <= 0 || H <= 0 || S <= 0 || T <= 0 || T > vlf::kMaxT || (D != 128 && D != 256) || !(p >= 0.f && p < 1.f))
+        return MSDA_E_BADARG;
+    if ((long long)B * S * H * D >= (1ll << 40) || (long long)B * H >= 65536 || S >= (1 << 30)) return MSDA_E_TOOLARGE;
+    return 0;
+}
+
+template <int D>
+cudaError_t vlf_forward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
+    cudaError_t e;
+    if ((e = cudaFuncSetAttribute(vlf::vlf_fwd_rows<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kFwdRowsSmem)) ||
+        (e = cudaFuncSetAttribute(vlf::vlf_fwd_cols<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kFwdColsSmem)))
+        return e;
+    const unsigned BH = (unsigned)(p.B * p.H);
+    vlf::vlf_fwd_rows<D><<<dim3(l.row_tiles, BH), vlf::kThreads, vlf::kFwdRowsSmem, st>>>(p);
+    vlf::vlf_colstats<<<BH, vlf::kMaxT, 0, st>>>(p, l.row_tiles);
+    vlf::vlf_fwd_cols<D><<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, vlf::kFwdColsSmem, st>>>(p);
+    vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part0, l.nsplit, (int)BH, p.H, p.T, D, p.out_l);
+    g_launches.fetch_add(4, std::memory_order_relaxed);
+    return cudaGetLastError();
+}
+
+template <int D>
+cudaError_t vlf_backward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
+    cudaError_t e;
+    if ((e = cudaFuncSetAttribute(vlf::vlf_bwd_rows<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kBwdRowsSmem)) ||
+        (e = cudaFuncSetAttribute(vlf::vlf_bwd_cols<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kBwdColsSmem)))
+        return e;
+    const unsigned BH = (unsigned)(p.B * p.H);
+    const long long rows = (long long)BH * (p.S + p.T);
+    vlf::vlf_bwd_delta<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(p, D);
+    vlf::vlf_bwd_rows<D><<<dim3(l.row_tiles, BH), vlf::kThreads, vlf::kBwdRowsSmem, st>>>(p);
+    vlf::vlf_bwd_cols<D><<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, vlf::kBwdColsSmem, st>>>(p);
+    vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part0, l.nsplit, (int)BH, p.H, p.T, D, p.dk);
+    vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part1, l.nsplit, (int)BH, p.H, p.T, D, p.dvl);
+    g_launches.fetch_add(5, std::memory_order_relaxed);
+    return cudaGetLastError();
+}
+
+bool all_aligned16(std::initializer_list<const void *> ptrs) {
+    for (const void *q : ptrs)
+        if (!q || !aligned16(q)) return false;
+    return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *bytes) {
+    if (!bytes) return MSDA_E_BADARG;
+    if (const int c = vlf_check(B, H, S, T, head_dim, 0.f)) return c;
+    *bytes = (int64_t)vlf_layout(B, H, S, T, head_dim).total;
+    return 0;
+}
+
+int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
+                            int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
+                            const int64_t *seed, float *out_v, float *out_l, float *stats, void *workspace,
+                            int64_t workspace_bytes, void *stream) {
+    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
+    if (!all_aligned16({q, k, v_v, v_l, out_v, out_l, stats, workspace}) || (dropout_p > 0.f && !seed)) return MSDA_E_BADARG;
+    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    vlf::Params p{};
+    p.q = q; p.k = k; p.vv = v_v; p.vl = v_l; p.bias = text_bias;
+    p.out_v = out_v; p.out_l = out_l;
+    p.rowstat = stats;
+    p.colstat = stats + (size_t)B * H * S * 2;
+    p.colpart = reinterpret_cast<float *>(ws + l.colpart);
+    p.part0 = reinterpret_cast<float *>(ws + l.part0);
+    p.seed = seed;
+    p.B = B; p.H = H; p.S = S; p.T = T;
+    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
+    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
+    p.split_rows = l.split_rows;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return (int)(head_dim == 128 ? vlf_forward_launch<128>(p, l, st) : vlf_forward_launch<256>(p, l, st));
+}
+
+int msda_vlfuse_backward_f32(const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
+                             const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
+                             const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
+                             int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
+                             float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
+                             void *stream) {
+    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
+    if (!all_aligned16({grad_out_v, grad_out_l, q, k, v_v, v_l, out_v, out_l, stats, grad_q, grad_k, grad_v_v, grad_v_l,
+                        workspace}) || (dropout_p > 0.f && !seed))
+        return MSDA_E_BADARG;
+    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    vlf::Params p{};
+    p.q = q; p.k = k; p.vv = v_v; p.vl = v_l; p.bias = text_bias;
+    p.dov = grad_out_v; p.dol = grad_out_l; p.ov = out_v; p.ol = out_l;
+    p.dq = grad_q; p.dk = grad_k; p.dvv = grad_v_v; p.dvl = grad_v_l;
+    p.rowstat = const_cast<float *>(stats);
+    p.colstat = const_cast<float *>(stats) + (size_t)B * H * S * 2;
+    p.part0 = reinterpret_cast<float *>(ws + l.part0);
+    p.part1 = reinterpret_cast<float *>(ws + l.part1);
+    p.delta_v = reinterpret_cast<float *>(ws + l.delta_v);
+    p.delta_l = reinterpret_cast<float *>(ws + l.delta_l);
+    p.seed = seed;
+    p.B = B; p.H = H; p.S = S; p.T = T;
+    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
+    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
+    p.split_rows = l.split_rows;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return (int)(head_dim == 128 ? vlf_backward_launch<128>(p, l, st) : vlf_backward_launch<256>(p, l, st));
+}
+
+int msda_vlfuse_dropout_mask_f32(const int64_t *seed, int B, int H, int S, int T, float dropout_p, float *mask_v,
+                                 float *mask_l, void *stream) {
+    if (!seed || !mask_v || !mask_l || B <= 0 || H <= 0 || S <= 0 || T <= 0 || !(dropout_p >= 0.f && dropout_p < 1.f))
+        return MSDA_E_BADARG;
+    const long long n = (long long)B * H * S * T;
+    const unsigned grid = (unsigned)((n + 255) / 256 < 65535 ? (n + 255) / 256 : 65535);
+    vlf::vlf_dropout_mask<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(seed, B * H, S, T, dropout_p, mask_v, mask_l);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return (int)cudaGetLastError();
 }
