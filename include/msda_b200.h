@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 6   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_* */
+#define MSDA_ABI_VERSION 7   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32 */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -274,7 +274,11 @@ int msda_linear_tf32_ws_ok(int N, int K);
  * allocated and nothing synchronises with the host; the calls can be captured into a CUDA graph.
  * msda_vlfuse_workspace: bytes of `workspace` both calls need for these sizes.
  * msda_vlfuse_backward_f32 writes all four gradients (overwritten, not accumulated).
- * msda_vlfuse_dropout_mask_f32: the keep decisions as 1.0 / 0.0, mask_v [B*H, S, T] (vision), mask_l [B*H, T, S] (text). */
+ * msda_vlfuse_dropout_mask_f32: the keep decisions as 1.0 / 0.0, mask_v [B*H, S, T] (vision), mask_l [B*H, T, S] (text).
+ * msda_vlfuse_forward_tf32 / _backward_tf32: the same calls with every S x T x d product on TF32 tensor cores (each
+ * operand rounded once to TF32, round to nearest; fp32 accumulation; everything between the products fp32 as above).
+ * Same workspace, stats layout, dropout masks, determinism and launch count.  A backward must use the mode of the
+ * forward that wrote `stats`. */
 int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *bytes);
 int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
                             int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
@@ -288,6 +292,16 @@ int msda_vlfuse_backward_f32(const float *grad_out_v, const float *grad_out_l, c
                              void *stream);
 int msda_vlfuse_dropout_mask_f32(const int64_t *seed, int B, int H, int S, int T, float dropout_p, float *mask_v,
                                  float *mask_l, void *stream);
+int msda_vlfuse_forward_tf32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
+                             int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
+                             const int64_t *seed, float *out_v, float *out_l, float *stats, void *workspace,
+                             int64_t workspace_bytes, void *stream);
+int msda_vlfuse_backward_tf32(const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
+                              const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
+                              const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
+                              int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
+                              float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
+                              void *stream);
 
 #ifdef __cplusplus
 }

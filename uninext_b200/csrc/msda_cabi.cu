@@ -15,6 +15,7 @@
 #include "msda_tmem.cuh"
 #include "msda_tiled.cuh"
 #include "msda_vlfuse.cuh"
+#include "msda_vlfuse_tc.cuh"
 
 namespace {
 
@@ -1153,32 +1154,39 @@ int vlf_check(int B, int H, int S, int T, int D, float p) {
     return 0;
 }
 
-template <int D>
+// TC: the TF32 tensor-core product kernels of msda_vlfuse_tc.cuh; the other kernels and the launch sequence are shared.
+template <int D, bool TC>
 cudaError_t vlf_forward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
+    auto rows = TC ? vlf::vlf_tc_fwd_rows<D> : vlf::vlf_fwd_rows<D>;
+    auto cols = TC ? vlf::vlf_tc_fwd_cols<D> : vlf::vlf_fwd_cols<D>;
+    const int rows_smem = TC ? vlf::kTcFwdRowsSmem : vlf::kFwdRowsSmem, cols_smem = TC ? vlf::kTcFwdColsSmem : vlf::kFwdColsSmem;
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(vlf::vlf_fwd_rows<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kFwdRowsSmem)) ||
-        (e = cudaFuncSetAttribute(vlf::vlf_fwd_cols<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kFwdColsSmem)))
+    if ((e = cudaFuncSetAttribute(rows, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem)) ||
+        (e = cudaFuncSetAttribute(cols, cudaFuncAttributeMaxDynamicSharedMemorySize, cols_smem)))
         return e;
     const unsigned BH = (unsigned)(p.B * p.H);
-    vlf::vlf_fwd_rows<D><<<dim3(l.row_tiles, BH), vlf::kThreads, vlf::kFwdRowsSmem, st>>>(p);
+    rows<<<dim3(l.row_tiles, BH), vlf::kThreads, rows_smem, st>>>(p);
     vlf::vlf_colstats<<<BH, vlf::kMaxT, 0, st>>>(p, l.row_tiles);
-    vlf::vlf_fwd_cols<D><<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, vlf::kFwdColsSmem, st>>>(p);
+    cols<<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, cols_smem, st>>>(p);
     vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part0, l.nsplit, (int)BH, p.H, p.T, D, p.out_l);
     g_launches.fetch_add(4, std::memory_order_relaxed);
     return cudaGetLastError();
 }
 
-template <int D>
+template <int D, bool TC>
 cudaError_t vlf_backward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
+    auto rows_k = TC ? vlf::vlf_tc_bwd_rows<D> : vlf::vlf_bwd_rows<D>;
+    auto cols_k = TC ? vlf::vlf_tc_bwd_cols<D> : vlf::vlf_bwd_cols<D>;
+    const int rows_smem = TC ? vlf::kTcBwdRowsSmem : vlf::kBwdRowsSmem, cols_smem = TC ? vlf::kTcBwdColsSmem : vlf::kBwdColsSmem;
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(vlf::vlf_bwd_rows<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kBwdRowsSmem)) ||
-        (e = cudaFuncSetAttribute(vlf::vlf_bwd_cols<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, vlf::kBwdColsSmem)))
+    if ((e = cudaFuncSetAttribute(rows_k, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem)) ||
+        (e = cudaFuncSetAttribute(cols_k, cudaFuncAttributeMaxDynamicSharedMemorySize, cols_smem)))
         return e;
     const unsigned BH = (unsigned)(p.B * p.H);
     const long long rows = (long long)BH * (p.S + p.T);
     vlf::vlf_bwd_delta<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, st>>>(p, D);
-    vlf::vlf_bwd_rows<D><<<dim3(l.row_tiles, BH), vlf::kThreads, vlf::kBwdRowsSmem, st>>>(p);
-    vlf::vlf_bwd_cols<D><<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, vlf::kBwdColsSmem, st>>>(p);
+    rows_k<<<dim3(l.row_tiles, BH), vlf::kThreads, rows_smem, st>>>(p);
+    cols_k<<<dim3(l.col_tiles, l.nsplit, BH), vlf::kThreads, cols_smem, st>>>(p);
     vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part0, l.nsplit, (int)BH, p.H, p.T, D, p.dk);
     vlf::vlf_reduce<<<dim3(p.T, BH), D, 0, st>>>(p.part1, l.nsplit, (int)BH, p.H, p.T, D, p.dvl);
     g_launches.fetch_add(5, std::memory_order_relaxed);
@@ -1202,10 +1210,10 @@ int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *byt
     return 0;
 }
 
-int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
-                            int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
-                            const int64_t *seed, float *out_v, float *out_l, float *stats, void *workspace,
-                            int64_t workspace_bytes, void *stream) {
+static int vlf_forward(bool tc, const float *q, const float *k, const float *v_v, const float *v_l,
+                       const float *text_bias, int B, int H, int S, int T, int head_dim, int clamp_min,
+                       int clamp_max, float dropout_p, const int64_t *seed, float *out_v, float *out_l, float *stats,
+                       void *workspace, int64_t workspace_bytes, void *stream) {
     if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
     if (!all_aligned16({q, k, v_v, v_l, out_v, out_l, stats, workspace}) || (dropout_p > 0.f && !seed)) return MSDA_E_BADARG;
     const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
@@ -1224,15 +1232,16 @@ int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, co
     p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
     p.split_rows = l.split_rows;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return (int)(head_dim == 128 ? vlf_forward_launch<128>(p, l, st) : vlf_forward_launch<256>(p, l, st));
+    if (tc) return (int)(head_dim == 128 ? vlf_forward_launch<128, true>(p, l, st) : vlf_forward_launch<256, true>(p, l, st));
+    return (int)(head_dim == 128 ? vlf_forward_launch<128, false>(p, l, st) : vlf_forward_launch<256, false>(p, l, st));
 }
 
-int msda_vlfuse_backward_f32(const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
-                             const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
-                             const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
-                             int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
-                             float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
-                             void *stream) {
+static int vlf_backward(bool tc, const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
+                        const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
+                        const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
+                        int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
+                        float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
+                        void *stream) {
     if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
     if (!all_aligned16({grad_out_v, grad_out_l, q, k, v_v, v_l, out_v, out_l, stats, grad_q, grad_k, grad_v_v, grad_v_l,
                         workspace}) || (dropout_p > 0.f && !seed))
@@ -1256,8 +1265,31 @@ int msda_vlfuse_backward_f32(const float *grad_out_v, const float *grad_out_l, c
     p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
     p.split_rows = l.split_rows;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return (int)(head_dim == 128 ? vlf_backward_launch<128>(p, l, st) : vlf_backward_launch<256>(p, l, st));
+    if (tc) return (int)(head_dim == 128 ? vlf_backward_launch<128, true>(p, l, st) : vlf_backward_launch<256, true>(p, l, st));
+    return (int)(head_dim == 128 ? vlf_backward_launch<128, false>(p, l, st) : vlf_backward_launch<256, false>(p, l, st));
 }
+
+// The public entries: one signature per direction, the mode as a flag.
+#define VLF_FORWARD_ARGS                                                                                                 \
+    const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias, int B, int H, int S,   \
+        int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *out_v,          \
+        float *out_l, float *stats, void *workspace, int64_t workspace_bytes, void *stream
+#define VLF_FORWARD_PASS q, k, v_v, v_l, text_bias, B, H, S, T, head_dim, clamp_min, clamp_max, dropout_p, seed, out_v, \
+                         out_l, stats, workspace, workspace_bytes, stream
+#define VLF_BACKWARD_ARGS                                                                                                \
+    const float *grad_out_v, const float *grad_out_l, const float *q, const float *k, const float *v_v,                \
+        const float *v_l, const float *text_bias, const float *out_v, const float *out_l, const float *stats, int B,    \
+        int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed,          \
+        float *grad_q, float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,       \
+        void *stream
+#define VLF_BACKWARD_PASS grad_out_v, grad_out_l, q, k, v_v, v_l, text_bias, out_v, out_l, stats, B, H, S, T, head_dim, \
+                          clamp_min, clamp_max, dropout_p, seed, grad_q, grad_k, grad_v_v, grad_v_l, workspace,         \
+                          workspace_bytes, stream
+
+int msda_vlfuse_forward_f32(VLF_FORWARD_ARGS) { return vlf_forward(false, VLF_FORWARD_PASS); }
+int msda_vlfuse_forward_tf32(VLF_FORWARD_ARGS) { return vlf_forward(true, VLF_FORWARD_PASS); }
+int msda_vlfuse_backward_f32(VLF_BACKWARD_ARGS) { return vlf_backward(false, VLF_BACKWARD_PASS); }
+int msda_vlfuse_backward_tf32(VLF_BACKWARD_ARGS) { return vlf_backward(true, VLF_BACKWARD_PASS); }
 
 int msda_vlfuse_dropout_mask_f32(const int64_t *seed, int B, int H, int S, int T, float dropout_p, float *mask_v,
                                  float *mask_l, void *stream) {

@@ -22,6 +22,7 @@ from torch.autograd.function import once_differentiable
 
 from uninext_b200 import _cabi
 from uninext_b200._determinism import deterministic_requested
+from uninext_b200._precision import tf32_allowed
 
 
 def _stream():
@@ -88,10 +89,10 @@ _AUTO_MASKED_TCGEN05 = _os.environ.get("MSDA_GEMM_AUTO_MASKED", "tcgen05") == "t
 
 def resolve_gemm(gemm: str) -> str:
     """"auto": the hand-written TF32 GEMM kernels when the caller has allowed TF32 products
-    (``torch.backends.cuda.matmul.allow_tf32`` -- the default of the PyTorch 1.10 stack the reference was trained with), cuBLAS
-    fp32 otherwise, so that strict-fp32 runs keep their 1e-4 parity with the reference."""
+    (``torch.backends.cuda.matmul.allow_tf32`` or ``fp32_precision = "tf32"`` -- the default of the PyTorch 1.10 stack the
+    reference was trained with), cuBLAS fp32 otherwise, so that strict-fp32 runs keep their 1e-4 parity with the reference."""
     if gemm == "auto":
-        return "tcgen05" if (torch.backends.cuda.matmul.allow_tf32 and _AUTO_TCGEN05) else "cublas"
+        return "tcgen05" if (tf32_allowed() and _AUTO_TCGEN05) else "cublas"
     return gemm
 
 
@@ -131,7 +132,7 @@ class _LinearColsum(Function):
         mask = row_mask.reshape(-1) if row_mask is not None else None
         # "auto" with a row mask: the fused kernel replaces GEMM + masked_fill (one launch instead of two), so it is taken
         # whenever TF32 products are allowed; without a mask cuBLAS is used.
-        fused_mask = gemm == "auto" and mask is not None and torch.backends.cuda.matmul.allow_tf32 and _AUTO_MASKED_TCGEN05
+        fused_mask = gemm == "auto" and mask is not None and tf32_allowed() and _AUTO_MASKED_TCGEN05
         if (resolve_gemm(gemm) == "tcgen05" or fused_mask) and tcgen05_ws_ok(x2, weight):
             y = tcgen05_linear_ex(x2, weight, bias, mask, relu)          # bias, padding-mask zeroing and ReLU in the epilogue
         elif relu:                                           # bias + ReLU in the cuBLASLt epilogue

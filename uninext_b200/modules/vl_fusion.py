@@ -4,7 +4,9 @@ weights load unchanged.
 
 The attention core -- logits, both clamps, the masked vision softmax, the text softmax, both dropouts and the two
 products -- runs in the fused CUDA kernels of msda_vlfuse.cuh (DESIGN.md section 3.11), which never store the
-[B*H, S, T] logits.  The six projections are cuBLAS GEMMs (``F.linear``).  ``vl_attention_torch`` restates the core
+[B*H, S, T] logits.  When torch allows TF32 matmuls (``allow_tf32``, ``set_float32_matmul_precision("high")`` or
+``fp32_precision = "tf32"``) the kernels of msda_vlfuse_tc.cuh run its products on TF32 tensor cores instead.  The six
+projections are cuBLAS GEMMs (``F.linear``).  ``vl_attention_torch`` restates the core
 with torch ops; it serves CPU tensors, ``stable_softmax_2d=True`` and shapes outside the kernels' limits
 (head_dim 128 / 256, T <= 256).
 """
@@ -17,6 +19,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import _cabi
+from .._precision import tf32_allowed
 from .deformable_layers import fp32_under_autocast
 
 MAX_TEXT_TOKENS = 256
@@ -99,10 +102,12 @@ def dropout_masks(seed, B, H, S, T, p):
 
 
 class VLAttentionFunction(torch.autograd.Function):
-    """Fused attention core: (q, k, vv, vl) in [B, L, H, d] -> (O_v, O_l).  Saves O(S + T) statistics per head."""
+    """Fused attention core: (q, k, vv, vl) in [B, L, H, d] -> (O_v, O_l).  Saves O(S + T) statistics per head.  ``tf32``
+    selects the tensor-core kernels; the backward runs in the forward's mode, since it recomputes the logits against the
+    statistics the forward saved."""
 
     @staticmethod
-    def forward(ctx, q, k, vv, vl, bias, clamp_min, clamp_max, dropout_p, seed):
+    def forward(ctx, q, k, vv, vl, bias, clamp_min, clamp_max, dropout_p, seed, tf32=False):
         q, k, vv, vl = (t.contiguous() for t in (q, k, vv, vl))
         B, S, H, D = q.shape
         T = k.shape[1]
@@ -110,41 +115,46 @@ class VLAttentionFunction(torch.autograd.Function):
         o_l = torch.empty_like(k)
         stats = torch.empty(B * H * (S + T) * 2, dtype=torch.float32, device=q.device)
         ws = _workspace(B, H, S, T, D, q.device)
-        _cabi.check(_cabi.load().msda_vlfuse_forward_f32(
+        name = "msda_vlfuse_forward_tf32" if tf32 else "msda_vlfuse_forward_f32"
+        _cabi.check(getattr(_cabi.load(), name)(
             _ptr(q), _ptr(k), _ptr(vv), _ptr(vl), _ptr(bias), B, H, S, T, D, int(clamp_min), int(clamp_max),
             ctypes.c_float(dropout_p), _ptr(seed), _ptr(o_v), _ptr(o_l), _ptr(stats), _ptr(ws), ws.numel(), _stream()),
-            "msda_vlfuse_forward_f32")
+            name)
         ctx.save_for_backward(q, k, vv, vl, bias, seed, o_v, o_l, stats)
-        ctx.cfg = (clamp_min, clamp_max, dropout_p)
+        ctx.cfg = (clamp_min, clamp_max, dropout_p, tf32)
         return o_v, o_l
 
     @staticmethod
     def backward(ctx, go_v, go_l):
         q, k, vv, vl, bias, seed, o_v, o_l, stats = ctx.saved_tensors
-        clamp_min, clamp_max, dropout_p = ctx.cfg
+        clamp_min, clamp_max, dropout_p, tf32 = ctx.cfg
         B, S, H, D = q.shape
         T = k.shape[1]
         go_v = torch.zeros_like(o_v) if go_v is None else go_v.contiguous()
         go_l = torch.zeros_like(o_l) if go_l is None else go_l.contiguous()
         dq, dk, dvv, dvl = (torch.empty_like(t) for t in (q, k, vv, vl))
         ws = _workspace(B, H, S, T, D, q.device)
-        _cabi.check(_cabi.load().msda_vlfuse_backward_f32(
+        name = "msda_vlfuse_backward_tf32" if tf32 else "msda_vlfuse_backward_f32"
+        _cabi.check(getattr(_cabi.load(), name)(
             _ptr(go_v), _ptr(go_l), _ptr(q), _ptr(k), _ptr(vv), _ptr(vl), _ptr(bias), _ptr(o_v), _ptr(o_l), _ptr(stats),
             B, H, S, T, D, int(clamp_min), int(clamp_max), ctypes.c_float(dropout_p), _ptr(seed), _ptr(dq), _ptr(dk),
-            _ptr(dvv), _ptr(dvl), _ptr(ws), ws.numel(), _stream()), "msda_vlfuse_backward_f32")
-        return dq, dk, dvv, dvl, None, None, None, None, None
+            _ptr(dvv), _ptr(dvl), _ptr(ws), ws.numel(), _stream()), name)
+        return dq, dk, dvv, dvl, None, None, None, None, None, None
 
 
 def vl_attention(q, k, vv, vl, bias=None, clamp_min=True, clamp_max=True, dropout_p=0.0, training=False,
                  stable_softmax_2d=False, seed=None):
     """The attention core, fused where ``fused_supported`` holds, else ``vl_attention_torch``.  ``seed`` (a CUDA int64
-    tensor of one element) keys the fused dropout; by default one is drawn with ``draw_seed``."""
+    tensor of one element) keys the fused dropout; by default one is drawn with ``draw_seed``.  The fused products run
+    on TF32 tensor cores when torch allows TF32 matmuls at the time of the forward (``tf32_allowed``), in fp32 otherwise;
+    the backward keeps the forward's mode."""
     if not fused_supported(q, k, stable_softmax_2d):
         return vl_attention_torch(q, k, vv, vl, bias, clamp_min, clamp_max, dropout_p, training, stable_softmax_2d)
     p = float(dropout_p) if training else 0.0
     if p > 0.0 and seed is None:
         seed = draw_seed(q.device)
-    return VLAttentionFunction.apply(q, k, vv, vl, bias, bool(clamp_min), bool(clamp_max), p, seed if p > 0.0 else None)
+    return VLAttentionFunction.apply(q, k, vv, vl, bias, bool(clamp_min), bool(clamp_max), p, seed if p > 0.0 else None,
+                                     tf32_allowed())
 
 
 def _fuse_flag(cfg, name, default):
