@@ -45,7 +45,8 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 7   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32 */
+#define MSDA_ABI_VERSION 8   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
+                                8: msda_vlfuse_*_bf16 */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -278,7 +279,11 @@ int msda_linear_tf32_ws_ok(int N, int K);
  * msda_vlfuse_forward_tf32 / _backward_tf32: the same calls with every S x T x d product on TF32 tensor cores (each
  * operand rounded once to TF32, round to nearest; fp32 accumulation; everything between the products fp32 as above).
  * Same workspace, stats layout, dropout masks, determinism and launch count.  A backward must use the mode of the
- * forward that wrote `stats`. */
+ * forward that wrote `stats`.
+ * msda_vlfuse_forward_bf16 / _backward_bf16: the same calls on bf16 tensors (uint16_t bit patterns) with every S x T x d
+ * product on bf16 tensor cores: P_v, P_l and dS rounded once to bf16 (round to nearest even), fp32 accumulation, every
+ * output rounded once to bf16.  text_bias and stats stay fp32.  Same workspace, alignment rule, dropout masks
+ * (msda_vlfuse_dropout_mask_f32), determinism and launch count. */
 int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *bytes);
 int msda_vlfuse_forward_f32(const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias,
                             int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p,
@@ -302,6 +307,16 @@ int msda_vlfuse_backward_tf32(const float *grad_out_v, const float *grad_out_l, 
                               int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
                               float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
                               void *stream);
+int msda_vlfuse_forward_bf16(const uint16_t *q, const uint16_t *k, const uint16_t *v_v, const uint16_t *v_l,
+                             const float *text_bias, int B, int H, int S, int T, int head_dim, int clamp_min, int clamp_max,
+                             float dropout_p, const int64_t *seed, uint16_t *out_v, uint16_t *out_l, float *stats,
+                             void *workspace, int64_t workspace_bytes, void *stream);
+int msda_vlfuse_backward_bf16(const uint16_t *grad_out_v, const uint16_t *grad_out_l, const uint16_t *q,
+                              const uint16_t *k, const uint16_t *v_v, const uint16_t *v_l, const float *text_bias,
+                              const uint16_t *out_v, const uint16_t *out_l, const float *stats, int B, int H, int S,
+                              int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed,
+                              uint16_t *grad_q, uint16_t *grad_k, uint16_t *grad_v_v, uint16_t *grad_v_l,
+                              void *workspace, int64_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }

@@ -56,8 +56,10 @@ SIGNATURES = {
     "msda_vlfuse_dropout_mask_f32": (_i, [_vp] + [_i] * 4 + [ctypes.c_float] + [_vp] * 3),
     "msda_vlfuse_forward_tf32": (_i, [_vp] * 5 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 4 + [ctypes.c_int64, _vp]),
     "msda_vlfuse_backward_tf32": (_i, [_vp] * 10 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 5 + [ctypes.c_int64, _vp]),
+    "msda_vlfuse_forward_bf16": (_i, [_vp] * 5 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 4 + [ctypes.c_int64, _vp]),
+    "msda_vlfuse_backward_bf16": (_i, [_vp] * 10 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 5 + [ctypes.c_int64, _vp]),
 }
-ABI_VERSION = 7
+ABI_VERSION = 8
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 

@@ -20,7 +20,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libmsda_b200.so")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
 SOURCES = ["msda_cabi.cu", "msda_gemm_sm90.cu"]
-HEADERS = ["msda_common.cuh", "msda_tiled.cuh", "msda_region.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh", "msda_det.cuh", "msda_vlfuse.cuh", "msda_vlfuse_tc.cuh"]
+HEADERS = ["msda_common.cuh", "msda_tiled.cuh", "msda_region.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh", "msda_det.cuh", "msda_vlfuse.cuh", "msda_vlfuse_tc.cuh", "msda_vlfuse_bf16.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -16,6 +16,7 @@
 #include "msda_tiled.cuh"
 #include "msda_vlfuse.cuh"
 #include "msda_vlfuse_tc.cuh"
+#include "msda_vlfuse_bf16.cuh"
 
 namespace {
 
@@ -1154,12 +1155,11 @@ int vlf_check(int B, int H, int S, int T, int D, float p) {
     return 0;
 }
 
-// TC: the TF32 tensor-core product kernels of msda_vlfuse_tc.cuh; the other kernels and the launch sequence are shared.
-template <int D, bool TC>
-cudaError_t vlf_forward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
-    auto rows = TC ? vlf::vlf_tc_fwd_rows<D> : vlf::vlf_fwd_rows<D>;
-    auto cols = TC ? vlf::vlf_tc_fwd_cols<D> : vlf::vlf_fwd_cols<D>;
-    const int rows_smem = TC ? vlf::kTcFwdRowsSmem : vlf::kFwdRowsSmem, cols_smem = TC ? vlf::kTcFwdColsSmem : vlf::kFwdColsSmem;
+// The launch sequence every mode shares: the mode's row-side and column-side product kernels around vlf_colstats,
+// vlf_reduce and vlf_bwd_delta.
+template <int D, class T>
+cudaError_t vlf_forward_launch(const vlf::ParamsT<T> &p, const VlfLayout &l, void (*rows)(vlf::ParamsT<T>), int rows_smem,
+                               void (*cols)(vlf::ParamsT<T>), int cols_smem, cudaStream_t st) {
     cudaError_t e;
     if ((e = cudaFuncSetAttribute(rows, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem)) ||
         (e = cudaFuncSetAttribute(cols, cudaFuncAttributeMaxDynamicSharedMemorySize, cols_smem)))
@@ -1173,11 +1173,9 @@ cudaError_t vlf_forward_launch(const vlf::Params &p, const VlfLayout &l, cudaStr
     return cudaGetLastError();
 }
 
-template <int D, bool TC>
-cudaError_t vlf_backward_launch(const vlf::Params &p, const VlfLayout &l, cudaStream_t st) {
-    auto rows_k = TC ? vlf::vlf_tc_bwd_rows<D> : vlf::vlf_bwd_rows<D>;
-    auto cols_k = TC ? vlf::vlf_tc_bwd_cols<D> : vlf::vlf_bwd_cols<D>;
-    const int rows_smem = TC ? vlf::kTcBwdRowsSmem : vlf::kBwdRowsSmem, cols_smem = TC ? vlf::kTcBwdColsSmem : vlf::kBwdColsSmem;
+template <int D, class T>
+cudaError_t vlf_backward_launch(const vlf::ParamsT<T> &p, const VlfLayout &l, void (*rows_k)(vlf::ParamsT<T>),
+                                int rows_smem, void (*cols_k)(vlf::ParamsT<T>), int cols_smem, cudaStream_t st) {
     cudaError_t e;
     if ((e = cudaFuncSetAttribute(rows_k, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem)) ||
         (e = cudaFuncSetAttribute(cols_k, cudaFuncAttributeMaxDynamicSharedMemorySize, cols_smem)))
@@ -1193,10 +1191,105 @@ cudaError_t vlf_backward_launch(const vlf::Params &p, const VlfLayout &l, cudaSt
     return cudaGetLastError();
 }
 
+// The product kernels of each mode: F32 (msda_vlfuse.cuh), TF32 (msda_vlfuse_tc.cuh), BF16 (msda_vlfuse_bf16.cuh).
+enum VlfMode { kVlfF32, kVlfTF32, kVlfBF16 };
+
+template <int D>
+cudaError_t vlf_forward_mode(const vlf::Params &p, const VlfLayout &l, VlfMode mode, cudaStream_t st) {
+    if (mode == kVlfTF32)
+        return vlf_forward_launch<D>(p, l, vlf::vlf_tc_fwd_rows<D>, vlf::kTcFwdRowsSmem, vlf::vlf_tc_fwd_cols<D>,
+                                     vlf::kTcFwdColsSmem, st);
+    return vlf_forward_launch<D>(p, l, vlf::vlf_fwd_rows<D>, vlf::kFwdRowsSmem, vlf::vlf_fwd_cols<D>, vlf::kFwdColsSmem, st);
+}
+template <int D>
+cudaError_t vlf_forward_mode(const vlf::ParamsH &p, const VlfLayout &l, VlfMode, cudaStream_t st) {
+    return vlf_forward_launch<D>(p, l, vlf::vlf_bf16_fwd_rows<D>, vlf::kH_FwdRowsSmem, vlf::vlf_bf16_fwd_cols<D>,
+                                 vlf::kH_FwdColsSmem, st);
+}
+template <int D>
+cudaError_t vlf_backward_mode(const vlf::Params &p, const VlfLayout &l, VlfMode mode, cudaStream_t st) {
+    if (mode == kVlfTF32)
+        return vlf_backward_launch<D>(p, l, vlf::vlf_tc_bwd_rows<D>, vlf::kTcBwdRowsSmem, vlf::vlf_tc_bwd_cols<D>,
+                                      vlf::kTcBwdColsSmem, st);
+    return vlf_backward_launch<D>(p, l, vlf::vlf_bwd_rows<D>, vlf::kBwdRowsSmem, vlf::vlf_bwd_cols<D>, vlf::kBwdColsSmem,
+                                  st);
+}
+template <int D>
+cudaError_t vlf_backward_mode(const vlf::ParamsH &p, const VlfLayout &l, VlfMode, cudaStream_t st) {
+    return vlf_backward_launch<D>(p, l, vlf::vlf_bf16_bwd_rows<D>, vlf::kH_BwdRowsSmem, vlf::vlf_bf16_bwd_cols<D>,
+                                  vlf::kH_BwdColsSmem, st);
+}
+
+// The tensors' element type behind an ABI pointer type: float, or bf16 passed as uint16_t.
+template <class A> struct VlfElem { using type = float; };
+template <> struct VlfElem<uint16_t> { using type = __nv_bfloat16; };
+
 bool all_aligned16(std::initializer_list<const void *> ptrs) {
     for (const void *q : ptrs)
         if (!q || !aligned16(q)) return false;
     return true;
+}
+
+template <class A>
+int vlf_forward(VlfMode mode, const A *q, const A *k, const A *v_v, const A *v_l, const float *text_bias, int B, int H,
+                int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, A *out_v,
+                A *out_l, float *stats, void *workspace, int64_t workspace_bytes, void *stream) {
+    using E = typename VlfElem<A>::type;
+    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
+    if (!all_aligned16({q, k, v_v, v_l, out_v, out_l, stats, workspace}) || (dropout_p > 0.f && !seed)) return MSDA_E_BADARG;
+    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    vlf::ParamsT<E> p{};
+    p.q = reinterpret_cast<const E *>(q); p.k = reinterpret_cast<const E *>(k);
+    p.vv = reinterpret_cast<const E *>(v_v); p.vl = reinterpret_cast<const E *>(v_l); p.bias = text_bias;
+    p.out_v = reinterpret_cast<E *>(out_v); p.out_l = reinterpret_cast<E *>(out_l);
+    p.rowstat = stats;
+    p.colstat = stats + (size_t)B * H * S * 2;
+    p.colpart = reinterpret_cast<float *>(ws + l.colpart);
+    p.part0 = reinterpret_cast<float *>(ws + l.part0);
+    p.seed = seed;
+    p.B = B; p.H = H; p.S = S; p.T = T;
+    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
+    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
+    p.split_rows = l.split_rows;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return (int)(head_dim == 128 ? vlf_forward_mode<128>(p, l, mode, st) : vlf_forward_mode<256>(p, l, mode, st));
+}
+
+template <class A>
+int vlf_backward(VlfMode mode, const A *grad_out_v, const A *grad_out_l, const A *q, const A *k, const A *v_v,
+                 const A *v_l, const float *text_bias, const A *out_v, const A *out_l, const float *stats, int B, int H,
+                 int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, A *grad_q,
+                 A *grad_k, A *grad_v_v, A *grad_v_l, void *workspace, int64_t workspace_bytes, void *stream) {
+    using E = typename VlfElem<A>::type;
+    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
+    if (!all_aligned16({grad_out_v, grad_out_l, q, k, v_v, v_l, out_v, out_l, stats, grad_q, grad_k, grad_v_v, grad_v_l,
+                        workspace}) || (dropout_p > 0.f && !seed))
+        return MSDA_E_BADARG;
+    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    vlf::ParamsT<E> p{};
+    p.q = reinterpret_cast<const E *>(q); p.k = reinterpret_cast<const E *>(k);
+    p.vv = reinterpret_cast<const E *>(v_v); p.vl = reinterpret_cast<const E *>(v_l); p.bias = text_bias;
+    p.dov = reinterpret_cast<const E *>(grad_out_v); p.dol = reinterpret_cast<const E *>(grad_out_l);
+    p.ov = reinterpret_cast<const E *>(out_v); p.ol = reinterpret_cast<const E *>(out_l);
+    p.dq = reinterpret_cast<E *>(grad_q); p.dk = reinterpret_cast<E *>(grad_k);
+    p.dvv = reinterpret_cast<E *>(grad_v_v); p.dvl = reinterpret_cast<E *>(grad_v_l);
+    p.rowstat = const_cast<float *>(stats);
+    p.colstat = const_cast<float *>(stats) + (size_t)B * H * S * 2;
+    p.part0 = reinterpret_cast<float *>(ws + l.part0);
+    p.part1 = reinterpret_cast<float *>(ws + l.part1);
+    p.delta_v = reinterpret_cast<float *>(ws + l.delta_v);
+    p.delta_l = reinterpret_cast<float *>(ws + l.delta_l);
+    p.seed = seed;
+    p.B = B; p.H = H; p.S = S; p.T = T;
+    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
+    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
+    p.split_rows = l.split_rows;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return (int)(head_dim == 128 ? vlf_backward_mode<128>(p, l, mode, st) : vlf_backward_mode<256>(p, l, mode, st));
 }
 
 }  // namespace
@@ -1210,86 +1303,28 @@ int msda_vlfuse_workspace(int B, int H, int S, int T, int head_dim, int64_t *byt
     return 0;
 }
 
-static int vlf_forward(bool tc, const float *q, const float *k, const float *v_v, const float *v_l,
-                       const float *text_bias, int B, int H, int S, int T, int head_dim, int clamp_min,
-                       int clamp_max, float dropout_p, const int64_t *seed, float *out_v, float *out_l, float *stats,
-                       void *workspace, int64_t workspace_bytes, void *stream) {
-    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
-    if (!all_aligned16({q, k, v_v, v_l, out_v, out_l, stats, workspace}) || (dropout_p > 0.f && !seed)) return MSDA_E_BADARG;
-    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
-    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
-    char *ws = static_cast<char *>(workspace);
-    vlf::Params p{};
-    p.q = q; p.k = k; p.vv = v_v; p.vl = v_l; p.bias = text_bias;
-    p.out_v = out_v; p.out_l = out_l;
-    p.rowstat = stats;
-    p.colstat = stats + (size_t)B * H * S * 2;
-    p.colpart = reinterpret_cast<float *>(ws + l.colpart);
-    p.part0 = reinterpret_cast<float *>(ws + l.part0);
-    p.seed = seed;
-    p.B = B; p.H = H; p.S = S; p.T = T;
-    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
-    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
-    p.split_rows = l.split_rows;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (tc) return (int)(head_dim == 128 ? vlf_forward_launch<128, true>(p, l, st) : vlf_forward_launch<256, true>(p, l, st));
-    return (int)(head_dim == 128 ? vlf_forward_launch<128, false>(p, l, st) : vlf_forward_launch<256, false>(p, l, st));
-}
-
-static int vlf_backward(bool tc, const float *grad_out_v, const float *grad_out_l, const float *q, const float *k,
-                        const float *v_v, const float *v_l, const float *text_bias, const float *out_v,
-                        const float *out_l, const float *stats, int B, int H, int S, int T, int head_dim,
-                        int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *grad_q,
-                        float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,
-                        void *stream) {
-    if (const int c = vlf_check(B, H, S, T, head_dim, dropout_p)) return c;
-    if (!all_aligned16({grad_out_v, grad_out_l, q, k, v_v, v_l, out_v, out_l, stats, grad_q, grad_k, grad_v_v, grad_v_l,
-                        workspace}) || (dropout_p > 0.f && !seed))
-        return MSDA_E_BADARG;
-    const VlfLayout l = vlf_layout(B, H, S, T, head_dim);
-    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
-    char *ws = static_cast<char *>(workspace);
-    vlf::Params p{};
-    p.q = q; p.k = k; p.vv = v_v; p.vl = v_l; p.bias = text_bias;
-    p.dov = grad_out_v; p.dol = grad_out_l; p.ov = out_v; p.ol = out_l;
-    p.dq = grad_q; p.dk = grad_k; p.dvv = grad_v_v; p.dvl = grad_v_l;
-    p.rowstat = const_cast<float *>(stats);
-    p.colstat = const_cast<float *>(stats) + (size_t)B * H * S * 2;
-    p.part0 = reinterpret_cast<float *>(ws + l.part0);
-    p.part1 = reinterpret_cast<float *>(ws + l.part1);
-    p.delta_v = reinterpret_cast<float *>(ws + l.delta_v);
-    p.delta_l = reinterpret_cast<float *>(ws + l.delta_l);
-    p.seed = seed;
-    p.B = B; p.H = H; p.S = S; p.T = T;
-    p.clamp_min = clamp_min != 0; p.clamp_max = clamp_max != 0;
-    p.p = dropout_p; p.keep_scale = 1.f / (1.f - dropout_p);
-    p.split_rows = l.split_rows;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (tc) return (int)(head_dim == 128 ? vlf_backward_launch<128, true>(p, l, st) : vlf_backward_launch<256, true>(p, l, st));
-    return (int)(head_dim == 128 ? vlf_backward_launch<128, false>(p, l, st) : vlf_backward_launch<256, false>(p, l, st));
-}
-
-// The public entries: one signature per direction, the mode as a flag.
-#define VLF_FORWARD_ARGS                                                                                                 \
-    const float *q, const float *k, const float *v_v, const float *v_l, const float *text_bias, int B, int H, int S,   \
-        int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, float *out_v,          \
-        float *out_l, float *stats, void *workspace, int64_t workspace_bytes, void *stream
+// The public entries: one signature per direction and element type, the mode as a flag.
+#define VLF_FORWARD_ARGS(A)                                                                                              \
+    const A *q, const A *k, const A *v_v, const A *v_l, const float *text_bias, int B, int H, int S, int T,            \
+        int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, A *out_v, A *out_l,           \
+        float *stats, void *workspace, int64_t workspace_bytes, void *stream
 #define VLF_FORWARD_PASS q, k, v_v, v_l, text_bias, B, H, S, T, head_dim, clamp_min, clamp_max, dropout_p, seed, out_v, \
                          out_l, stats, workspace, workspace_bytes, stream
-#define VLF_BACKWARD_ARGS                                                                                                \
-    const float *grad_out_v, const float *grad_out_l, const float *q, const float *k, const float *v_v,                \
-        const float *v_l, const float *text_bias, const float *out_v, const float *out_l, const float *stats, int B,    \
-        int H, int S, int T, int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed,          \
-        float *grad_q, float *grad_k, float *grad_v_v, float *grad_v_l, void *workspace, int64_t workspace_bytes,       \
-        void *stream
+#define VLF_BACKWARD_ARGS(A)                                                                                             \
+    const A *grad_out_v, const A *grad_out_l, const A *q, const A *k, const A *v_v, const A *v_l,                      \
+        const float *text_bias, const A *out_v, const A *out_l, const float *stats, int B, int H, int S, int T,          \
+        int head_dim, int clamp_min, int clamp_max, float dropout_p, const int64_t *seed, A *grad_q, A *grad_k,         \
+        A *grad_v_v, A *grad_v_l, void *workspace, int64_t workspace_bytes, void *stream
 #define VLF_BACKWARD_PASS grad_out_v, grad_out_l, q, k, v_v, v_l, text_bias, out_v, out_l, stats, B, H, S, T, head_dim, \
                           clamp_min, clamp_max, dropout_p, seed, grad_q, grad_k, grad_v_v, grad_v_l, workspace,         \
                           workspace_bytes, stream
 
-int msda_vlfuse_forward_f32(VLF_FORWARD_ARGS) { return vlf_forward(false, VLF_FORWARD_PASS); }
-int msda_vlfuse_forward_tf32(VLF_FORWARD_ARGS) { return vlf_forward(true, VLF_FORWARD_PASS); }
-int msda_vlfuse_backward_f32(VLF_BACKWARD_ARGS) { return vlf_backward(false, VLF_BACKWARD_PASS); }
-int msda_vlfuse_backward_tf32(VLF_BACKWARD_ARGS) { return vlf_backward(true, VLF_BACKWARD_PASS); }
+int msda_vlfuse_forward_f32(VLF_FORWARD_ARGS(float)) { return vlf_forward(kVlfF32, VLF_FORWARD_PASS); }
+int msda_vlfuse_forward_tf32(VLF_FORWARD_ARGS(float)) { return vlf_forward(kVlfTF32, VLF_FORWARD_PASS); }
+int msda_vlfuse_forward_bf16(VLF_FORWARD_ARGS(uint16_t)) { return vlf_forward(kVlfBF16, VLF_FORWARD_PASS); }
+int msda_vlfuse_backward_f32(VLF_BACKWARD_ARGS(float)) { return vlf_backward(kVlfF32, VLF_BACKWARD_PASS); }
+int msda_vlfuse_backward_tf32(VLF_BACKWARD_ARGS(float)) { return vlf_backward(kVlfTF32, VLF_BACKWARD_PASS); }
+int msda_vlfuse_backward_bf16(VLF_BACKWARD_ARGS(uint16_t)) { return vlf_backward(kVlfBF16, VLF_BACKWARD_PASS); }
 
 int msda_vlfuse_dropout_mask_f32(const int64_t *seed, int B, int H, int S, int T, float dropout_p, float *mask_v,
                                  float *mask_l, void *stream) {

@@ -15,6 +15,7 @@
 // ones.  Tensors are [B, L, H, d] (the Linear outputs viewed per head), rows of H*d floats.
 #pragma once
 
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -29,12 +30,15 @@ constexpr int kRowTile = 64;       // image tokens per row-side CTA
 constexpr int kColTile = 32;       // text tokens per column-side CTA
 constexpr float kClampAbs = 50000.f;
 
-struct Params {
-    const float *q, *k, *vv, *vl;          // [B,S,H,d], [B,T,H,d], [B,S,H,d], [B,T,H,d]
+// E: the element type of the tensors in [B, L, H, d] layout (float, or __nv_bfloat16 in bf16 mode); the text bias, the
+// statistics, the partial slots and the deltas are fp32 in every mode.
+template <class E>
+struct ParamsT {
+    const E *q, *k, *vv, *vl;              // [B,S,H,d], [B,T,H,d], [B,S,H,d], [B,T,H,d]
     const float *bias;                     // [B,T] additive text mask, or null
-    const float *dov, *dol, *ov, *ol;      // backward: grad_out / out, shapes of O_v [B,S,H,d] and O_l [B,T,H,d]
-    float *out_v, *out_l;
-    float *dq, *dk, *dvv, *dvl;
+    const E *dov, *dol, *ov, *ol;          // backward: grad_out / out, shapes of O_v [B,S,H,d] and O_l [B,T,H,d]
+    E *out_v, *out_l;
+    E *dq, *dk, *dvv, *dvl;
     float *rowstat;                        // [BH, S, 2]: (max, sum of exp) of the vision softmax of each image token
     float *colstat;                        // [BH, T, 2]: (max, sum of exp) over S of the clamped logits of each text token
     float *colpart;                        // [BH, row tiles, T, 2]: per-tile column partials of the forward
@@ -46,6 +50,12 @@ struct Params {
     float p, keep_scale;                   // dropout probability and 1 / (1 - p)
     int split_rows;                        // image tokens per column-side CTA (a multiple of kChunkS)
 };
+using Params = ParamsT<float>;
+
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ void store_as(float *dst, float v) { *dst = v; }
+__device__ __forceinline__ void store_as(__nv_bfloat16 *dst, float v) { *dst = __float2bfloat16_rn(v); }
 
 // ---- dropout: counter-based Philox4x32-10 keyed by (seed, direction, b*H + h, s, t) -------------------------------------
 __device__ __forceinline__ uint32_t philox_first(uint64_t seed, uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) {
@@ -69,13 +79,15 @@ __device__ __forceinline__ bool vlf_keep(uint64_t seed, uint32_t dir, uint32_t b
     return (float)(philox_first(seed, s, t, bh, dir) >> 8) * 5.9604644775390625e-8f >= p;
 }
 
-__device__ __forceinline__ float clamp_logit(float x, const Params &p) {
+template <class P>
+__device__ __forceinline__ float clamp_logit(float x, const P &p) {
     if (p.clamp_min) x = fmaxf(x, -kClampAbs);
     if (p.clamp_max) x = fminf(x, kClampAbs);
     return x;
 }
 // torch.clamp passes the gradient where min <= x <= max (inclusive).
-__device__ __forceinline__ bool clamp_passes(float x, const Params &p) {
+template <class P>
+__device__ __forceinline__ bool clamp_passes(float x, const P &p) {
     return (!p.clamp_min || x >= -kClampAbs) && (!p.clamp_max || x <= kClampAbs);
 }
 
@@ -304,7 +316,8 @@ __global__ void __launch_bounds__(kThreads, 1) vlf_fwd_rows(Params p) {
 }
 
 // Column statistics over all S: max, and sum of exp(x - max) rescaled from the tile partials in tile order.
-__global__ void vlf_colstats(Params p, int tiles) {
+template <class E>
+__global__ void vlf_colstats(ParamsT<E> p, int tiles) {
     const int bh = blockIdx.x, t = threadIdx.x;
     if (t >= p.T) return;
     const float *src = p.colpart + ((long)bh * tiles * p.T + t) * 2;
@@ -371,19 +384,23 @@ __global__ void __launch_bounds__(kThreads, 1) vlf_fwd_cols(Params p) {
             for (int j = 0; j < D / 32; ++j) dst[(ty * 4 + i) * D + tx + 32 * j] = o[i][j];
 }
 
-// out[b, t, h, :] = sum over ranges, in range order, of part[range, b*H + h, t, :].  One CTA per (t, b*H + h), D threads.
-__global__ void vlf_reduce(const float *part, int nsplit, int BH, int H, int T, int D, float *out) {
+// out[b, t, h, :] = sum over ranges, in range order, of part[range, b*H + h, t, :], rounded once to OutT.  One CTA per
+// (t, b*H + h), D threads.
+template <class OutT>
+__global__ void vlf_reduce(const float *part, int nsplit, int BH, int H, int T, int D, OutT *out) {
     const int t = blockIdx.x, bh = blockIdx.y, n = threadIdx.x;
     const long step = (long)BH * T * D;
     const float *src = part + ((long)bh * T + t) * D + n;
     float acc = 0.f;
     for (int i = 0; i < nsplit; ++i) acc += src[i * step];
-    out[(((long)(bh / H) * T + t) * H + bh % H) * D + n] = acc;
+    store_as(out + (((long)(bh / H) * T + t) * H + bh % H) * D + n, acc);
 }
 
 // ---- backward ---------------------------------------------------------------------------------------------------------
-// delta_v[bh, s] = dO_v . O_v and delta_l[bh, t] = dO_l . O_l; one warp per row, lanes combined in a fixed butterfly.
-__global__ void vlf_bwd_delta(Params p, int D) {
+// delta_v[bh, s] = dO_v . O_v and delta_l[bh, t] = dO_l . O_l in fp32; one warp per row, lanes combined in a fixed
+// butterfly.
+template <class E>
+__global__ void vlf_bwd_delta(ParamsT<E> p, int D) {
     const long rows_v = (long)p.B * p.H * p.S, rows = rows_v + (long)p.B * p.H * p.T;
     const long g = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -393,9 +410,9 @@ __global__ void vlf_bwd_delta(Params p, int D) {
     const int L = vis ? p.S : p.T;
     const int bh = (int)(gi / L), i = (int)(gi % L), b = bh / p.H, h = bh % p.H;
     const long off = (((long)b * L + i) * p.H + h) * D;
-    const float *go = (vis ? p.dov : p.dol) + off, *o = (vis ? p.ov : p.ol) + off;
+    const E *go = (vis ? p.dov : p.dol) + off, *o = (vis ? p.ov : p.ol) + off;
     float acc = 0.f;
-    for (int n = lane; n < D; n += 32) acc = fmaf(go[n], o[n], acc);
+    for (int n = lane; n < D; n += 32) acc = fmaf(to_f32(go[n]), to_f32(o[n]), acc);
     acc = warp_sum(acc);
     if (lane == 0) (vis ? p.delta_v : p.delta_l)[gi] = acc;
 }

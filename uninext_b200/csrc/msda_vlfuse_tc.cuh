@@ -38,10 +38,12 @@ constexpr int kTcBwdRowsSmem = (kRowTile * kLds + kMaxT * kLds + 2 * kRowTile * 
 constexpr int kTcBwdColsSmem = (kChunkS * kLds + kColTile * kLds + 3 * kChunkS * kLdq + 4 * kColTile + 3 * kChunkS) * 4;
 
 // ---- per-element maths shared by the four kernels ---------------------------------------------------------------------
-__device__ __forceinline__ float vis_logit(float x, float bias, const Params &p) { return p.bias ? x + bias : x; }
+template <class P>
+__device__ __forceinline__ float vis_logit(float x, float bias, const P &p) { return p.bias ? x + bias : x; }
 __device__ __forceinline__ float vis_prob(float xb, float m, float sum) { return expf(xb - m) / sum; }
 __device__ __forceinline__ float txt_prob(float x, float cm, float cs) { return expf(x - cm) / cs; }
-__device__ __forceinline__ float keep_scale(bool keep, float v, const Params &p) {
+template <class P>
+__device__ __forceinline__ float keep_scale(bool keep, float v, const P &p) {
     return keep ? v * (p.p > 0.f ? p.keep_scale : 1.f) : 0.f;
 }
 
