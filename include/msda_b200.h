@@ -45,8 +45,8 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 8   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
-                                8: msda_vlfuse_*_bf16 */
+#define MSDA_ABI_VERSION 9   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
+                                8: msda_vlfuse_*_bf16; 9: msda_mask_paste_f32 */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -246,6 +246,24 @@ int msda_condinst_backward_f32(const float *grad_logits, const float *feats, con
 int msda_aligned_bilinear_forward_f32(const float *in, int64_t planes, int h, int w, int factor, float *out, void *stream);
 int msda_aligned_bilinear_backward_f32(const float *grad_out, int64_t planes, int h, int w, int factor, float *grad_in,
                                        void *stream);
+
+/* ---- mask pasting for inference (DESIGN.md section 3.12, row f-5; uninext_img.py:474-479 + ddetrs.py:1060-1064,
+ * uninext_vid.py:620-622,1187-1192,1264-1266,1335-1337,1428-1431) -------------------------------------------------------
+ * msda_mask_paste_f32: logits [I, Hs, Ws] fp32 at `stride` -> out [I, out_h, out_w], the reference's chain
+ *     F.interpolate(bilinear, size=(stride*Hs, stride*Ws), align_corners=False) -> sigmoid [-> > threshold]
+ *     -> crop [:crop_h, :crop_w] -> F.interpolate(nearest, size=(out_h, out_w))
+ *   in one launch that writes nothing but `out`.  For output pixel (Y, X):
+ *     1. y' = min((int)floorf(Y * ((float)crop_h / out_h)), crop_h - 1), x' likewise (torch's `nearest`);
+ *     2. r = (float)Hs / (stride*Hs), src = max(r*(y' + 0.5) - 0.5, 0), i0 = (int)src, i1 = i0 + (i0 < Hs - 1),
+ *        lambda = src - i0; x likewise; v = the weighted sum of the four taps (upsample_bilinear2d, align_corners=False);
+ *     3. p = 1 / (1 + exp(-v)) in fp32;
+ *     4. binary == 0: out is fp32 and receives p; binary != 0: out is uint8 and receives p > threshold (strict) as 0 / 1.
+ *   Thresholding and nearest selection commute, so the image path (threshold first) and the video path (threshold last)
+ *   are both this call.  1 <= crop_h <= stride*Hs, 1 <= crop_w <= stride*Ws, out_h, out_w >= 1, I >= 0 (0: no launch);
+ *   otherwise MSDA_E_BADARG.  MSDA_E_TOOLARGE if out_h > 1048560 or out_w >= 2^30.  Offsets are 64-bit.  Nothing is
+ *   allocated and nothing synchronises with the host; the call can be captured into a CUDA graph. */
+int msda_mask_paste_f32(const float *logits, int64_t I, int Hs, int Ws, int stride, int crop_h, int crop_w, int out_h,
+                        int out_w, float threshold, int binary, void *out, void *stream);
 
 /* ---- TF32 GEMM for the Linears that bracket the op:  C[M,N] = A[M,K] . W[N,K]^T + bias[N]  (fp32 storage, sm_90 wgmma TF32
  * MMA with fp32 accumulation; TMA-fed).  K % 32 == 0, N % 32 == 0 (N % 64 == 0 above 256), N <= 512.

@@ -9,6 +9,7 @@
 #include "msda_condinst.cuh"
 #include "msda_det.cuh"
 #include "msda_generic.cuh"
+#include "msda_maskpaste.cuh"
 #include "msda_module.cuh"
 #include "msda_region.cuh"
 #include "msda_slab.cuh"
@@ -1051,6 +1052,34 @@ int msda_aligned_bilinear_backward_f32(const float *grad_out, int64_t planes, in
     const bool vec = w % 2 == 0 && (reinterpret_cast<uintptr_t>(grad_out) & 15) == 0 && (reinterpret_cast<uintptr_t>(grad_in) & 7) == 0;
     if (factor == 2 && vec) msda::aligned_bilinear2_bwd<<<grid, 256, 0, st>>>(grad_out, h, w, grad_in);
     else msda::aligned_bilinear_bwd<0><<<grid, 256, 0, st>>>(grad_out, h, w, factor, grad_in);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)cudaGetLastError();
+}
+
+int msda_mask_paste_f32(const float *logits, int64_t I, int Hs, int Ws, int stride, int crop_h, int crop_w, int out_h,
+                        int out_w, float threshold, int binary, void *out, void *stream) {
+    if (!logits || !out || I < 0 || Hs <= 0 || Ws <= 0 || stride <= 0 || crop_h <= 0 || crop_w <= 0 || out_h <= 0 ||
+        out_w <= 0 || (long long)stride * Hs >= (1ll << 31) || (long long)stride * Ws >= (1ll << 31) ||
+        crop_h > stride * Hs || crop_w > stride * Ws)
+        return MSDA_E_BADARG;
+    constexpr int cols = msda::kMpGroups * msda::kMpCols, rows = msda::kMpRows;
+    if (out_h > 65535 * rows || out_w >= (1 << 30)) return MSDA_E_TOOLARGE;
+    if (I == 0) return 0;
+    // The scales exactly as torch forms them for an explicit output size: (float)input_size / output_size.
+    const float near_y = (float)crop_h / (float)out_h, near_x = (float)crop_w / (float)out_w;
+    const float lin_y = (float)Hs / (float)(stride * Hs), lin_x = (float)Ws / (float)(stride * Ws);
+    const long long chunks = (I + msda::kMpInst - 1) / msda::kMpInst;
+    const dim3 grid((unsigned)((out_w + cols - 1) / cols), (unsigned)((out_h + rows - 1) / rows),
+                    (unsigned)(chunks < 65535 ? chunks : 65535));
+    const dim3 block(msda::kMpGroups, rows);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool vec = aligned16(out) && out_w % (binary ? msda::kMpCols : 4) == 0;
+#define MP_LAUNCH(B, V)                                                                                                  \
+    msda::mask_paste<B, V><<<grid, block, 0, st>>>(logits, I, Hs, Ws, crop_h, crop_w, out_h, out_w, near_y, near_x,   \
+                                                   lin_y, lin_x, threshold, out)
+    if (binary) { if (vec) MP_LAUNCH(true, true); else MP_LAUNCH(true, false); }
+    else { if (vec) MP_LAUNCH(false, true); else MP_LAUNCH(false, false); }
+#undef MP_LAUNCH
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return (int)cudaGetLastError();
 }
