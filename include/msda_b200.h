@@ -45,8 +45,8 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 9   /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
-                                8: msda_vlfuse_*_bf16; 9: msda_mask_paste_f32 */
+#define MSDA_ABI_VERSION 10  /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
+                                8: msda_vlfuse_*_bf16; 9: msda_mask_paste_f32; 10: msda_detpost_* */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -264,6 +264,40 @@ int msda_aligned_bilinear_backward_f32(const float *grad_out, int64_t planes, in
  *   allocated and nothing synchronises with the host; the call can be captured into a CUDA graph. */
 int msda_mask_paste_f32(const float *logits, int64_t I, int Hs, int Ws, int stride, int crop_h, int crop_w, int out_h,
                         int out_w, float threshold, int binary, void *out, void *stream);
+
+/* ---- detection post-processing for inference (DESIGN.md section 3.13, row f-6; uninext_img.py:367-485,
+ * uninext_vid.py:1092-1197) ----------------------------------------------------------------------------------------------
+ * msda_detpost_f32: box_cls [B, Q, T] fp32 token logits, box_pred [B, Q, 4] normalised cxcywh, iou_pred [B, Q] or NULL,
+ *   the positive map as CSR on the device (class c, 0-based, owns tokens[class_start[c] .. class_start[c+1]), int32),
+ *   image_sizes [B, 2] int32 (h, w) on the device.  For image b:
+ *     1. logit[q, c] = (fp32 sum of box_cls[b, q, tokens[j]] in CSR order) * ((float)1 / n_c)  (torch's CUDA mean);
+ *        prob = 1 / (1 + exp(-logit)) in fp32; with iou_pred, prob = sqrtf(prob * sigmoid(iou_pred[b, q])).
+ *     2. nms != 0 (the OTA branch, torchvision.ops.batched_nms's coordinate trick): score, class = max / argmax of prob
+ *        over c (lowest c on ties); boxes xyxy = (x_c - 0.5*w, y_c - 0.5*h, x_c + 0.5*w, y_c + 0.5*h); m = max of the
+ *        4Q coordinates; each coordinate += class * (m + 1); stable sort by score descending (ties: lower q first);
+ *        greedy: a later box is dropped when inter / (area_a + area_b - inter) > nms_iou, written in the order of
+ *        torchvision's devIoU source with every operation rounded once (no FMA contraction; torchvision's compiled
+ *        kernel may contract, so decisions within about an ulp of the threshold can differ from it).
+ *        K = the kept queries in that order.
+ *        nms == 0: K = all Q in query order.
+ *     3. top-k of the K*C pairs (kept rank r, class c): higher prob first, ties to the lower r * C + c;
+ *        count[b] = min(max_num_inst, K*C).
+ *     4. for j < count[b]: scores[b, j] = prob, labels[b, j] = c, query_index[b, j] = q (into the original Q),
+ *        boxes[b, j] = the xyxy box of q times (w, h, w, h).  j >= count[b]: scores 0, labels -1, query_index -1,
+ *        boxes 0.  All outputs are [B, max_num_inst] (boxes [B, max_num_inst, 4], 16-byte aligned), count is [B].
+ *   Two launches for the whole batch, whatever B, Q, C and nms.  Limits: 0 <= B <= 65535 (0: no launch), 1 <= Q <= 1024,
+ *   1 <= T <= 256, 1 <= C <= 4096, 1 <= max_num_inst <= Q*C, workspace_bytes >= msda_detpost_workspace(...), the
+ *   workspace 16-byte aligned; otherwise MSDA_E_BADARG.  Token indices must be < T and every class must own at least one
+ *   token: the call cannot read the device-side map before launching, so it does not check them (a token >= T makes
+ *   its class's probability NaN).  Offsets are 64-bit.  Nothing is allocated and nothing synchronises with the host;
+ *   the call can be captured into a CUDA graph.
+ * msda_detpost_workspace: the workspace bytes of a call with these sizes (prob [B, Q, C], the per-query maxima, and a
+ *   sort buffer when max_num_inst > 2048). */
+int msda_detpost_workspace(int B, int Q, int T, int C, int max_num_inst, int64_t *bytes);
+int msda_detpost_f32(const float *box_cls, const float *box_pred, const float *iou_pred, const int *class_start,
+                     const int *tokens, const int *image_sizes, int B, int Q, int T, int C, int nms, float nms_iou,
+                     int max_num_inst, float *scores, int *labels, int *query_index, float *boxes, int *count,
+                     void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---- TF32 GEMM for the Linears that bracket the op:  C[M,N] = A[M,K] . W[N,K]^T + bias[N]  (fp32 storage, sm_90 wgmma TF32
  * MMA with fp32 accumulation; TMA-fed).  K % 32 == 0, N % 32 == 0 (N % 64 == 0 above 256), N <= 512.

@@ -8,6 +8,7 @@
 #include "../../include/msda_b200.h"
 #include "msda_condinst.cuh"
 #include "msda_det.cuh"
+#include "msda_detpost.cuh"
 #include "msda_generic.cuh"
 #include "msda_maskpaste.cuh"
 #include "msda_module.cuh"
@@ -1081,6 +1082,93 @@ int msda_mask_paste_f32(const float *logits, int64_t I, int Hs, int Ws, int stri
     else { if (vec) MP_LAUNCH(false, true); else MP_LAUNCH(false, false); }
 #undef MP_LAUNCH
     g_launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)cudaGetLastError();
+}
+
+}  // extern "C"
+
+// ---- detection post-processing (f-6) ----------------------------------------------------------------------------------
+namespace {
+
+struct DetpostLayout {
+    size_t prob, qmax, qarg, sort, total;
+    long long sort_cap;                         // u64 sort slots per image in the workspace (0: the CTA sorts on chip)
+};
+
+inline size_t dp_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+int detpost_check(int B, int Q, int T, int C, int max_num_inst) {
+    if (B < 0 || B > 65535 || Q < 1 || Q > msda::kDpMaxQ || T < 1 || T > msda::kDpMaxT || C < 1 || C > msda::kDpMaxC ||
+        max_num_inst < 1 || (long long)max_num_inst > (long long)Q * C)
+        return MSDA_E_BADARG;
+    return 0;
+}
+
+DetpostLayout detpost_layout(int B, int Q, int C, int max_num_inst) {
+    DetpostLayout l{};
+    long long p = 1;
+    while (p < max_num_inst) p <<= 1;
+    l.sort_cap = p > msda::kDpSmemSort ? p : 0;
+    l.prob = 0;
+    l.qmax = dp_align(l.prob + (size_t)B * Q * C * sizeof(float));
+    l.qarg = dp_align(l.qmax + (size_t)B * Q * sizeof(float));
+    l.sort = dp_align(l.qarg + (size_t)B * Q * sizeof(int));
+    l.total = dp_align(l.sort + (size_t)B * l.sort_cap * sizeof(unsigned long long));
+    return l;
+}
+
+}  // namespace
+
+extern "C" {
+
+int msda_detpost_workspace(int B, int Q, int T, int C, int max_num_inst, int64_t *bytes) {
+    if (!bytes) return MSDA_E_BADARG;
+    if (const int c = detpost_check(B, Q, T, C, max_num_inst)) return c;
+    *bytes = (int64_t)detpost_layout(B, Q, C, max_num_inst).total;
+    return 0;
+}
+
+int msda_detpost_f32(const float *box_cls, const float *box_pred, const float *iou_pred, const int *class_start,
+                     const int *tokens, const int *image_sizes, int B, int Q, int T, int C, int nms, float nms_iou,
+                     int max_num_inst, float *scores, int *labels, int *query_index, float *boxes, int *count,
+                     void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!box_cls || !box_pred || !class_start || !tokens || !image_sizes || !scores || !labels || !query_index ||
+        !boxes || !count || !workspace || !aligned16(boxes) || !aligned16(workspace))
+        return MSDA_E_BADARG;
+    if (const int c = detpost_check(B, Q, T, C, max_num_inst)) return c;
+    const DetpostLayout l = detpost_layout(B, Q, C, max_num_inst);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    if (B == 0) return 0;
+    char *ws = static_cast<char *>(workspace);
+    float *prob = reinterpret_cast<float *>(ws + l.prob), *qmax = reinterpret_cast<float *>(ws + l.qmax);
+    int *qarg = reinterpret_cast<int *>(ws + l.qarg);
+    unsigned long long *sort_ws = reinterpret_cast<unsigned long long *>(ws + l.sort);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 sgrid((unsigned)((Q + msda::kDpScoreWarps - 1) / msda::kDpScoreWarps), (unsigned)B);
+    msda::detpost_scores<<<sgrid, msda::kDpScoreWarps * 32, 0, st>>>(box_cls, iou_pred, class_start, tokens, Q, T, C,
+                                                                     prob, qmax, qarg);
+    if (nms) {
+        // The opt-in is set once per device, to the Q = kDpMaxQ size, so no call can lower it under another's launch.
+        constexpr int kDynMax = msda::kDpMaxQ * (int)sizeof(float4) +
+                                msda::kDpMaxQ * ((msda::kDpMaxQ + 63) / 64) * (int)sizeof(unsigned long long);
+        static std::atomic<bool> opted_in[kMaxDevices];
+        const int dev = current_device();
+        if (!opted_in[dev].load(std::memory_order_acquire)) {
+            const cudaError_t e = cudaFuncSetAttribute(msda::detpost_select<true>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, kDynMax);
+            if (e != cudaSuccess) return (int)e;
+            opted_in[dev].store(true, std::memory_order_release);
+        }
+        const size_t dyn = (size_t)Q * sizeof(float4) + (size_t)Q * ((Q + 63) / 64) * sizeof(unsigned long long);
+        msda::detpost_select<true><<<B, msda::kDpThreads, dyn, st>>>(box_pred, image_sizes, prob, qmax, qarg, Q, C,
+                                                                     nms_iou, max_num_inst, l.sort_cap, sort_ws, scores,
+                                                                     labels, query_index, boxes, count);
+    } else {
+        msda::detpost_select<false><<<B, msda::kDpThreads, 0, st>>>(box_pred, image_sizes, prob, qmax, qarg, Q, C,
+                                                                    nms_iou, max_num_inst, l.sort_cap, sort_ws, scores,
+                                                                    labels, query_index, boxes, count);
+    }
+    g_launches.fetch_add(2, std::memory_order_relaxed);
     return (int)cudaGetLastError();
 }
 

@@ -1,0 +1,152 @@
+"""Detection post-processing for UNINEXT inference (DESIGN.md section 3.13, row f-6): grounding logits -> class scores ->
+class-aware NMS -> top-k boxes, scores and labels for the whole batch in two kernel launches
+(uninext_b200/csrc/msda_detpost.cuh, ``msda_detpost_f32``).
+
+Every image-style inference call of the reference runs, per image in a Python loop (``uninext_img.py:393-472``, and its
+copy ``uninext_vid.py:1092-1197``):
+
+    logits = convert_grounding_to_od_logits(box_cls[i], C, positive_map)   # a Python loop over the classes
+    prob = logits.sigmoid(); prob = sqrt(prob * iou_pred[i].sigmoid())      # with the IoU branch
+    keep = batched_nms(box_cxcywh_to_xyxy(box_pred[i]), *prob.max(1), 0.7)  # OTA on; a keep list of host-known length
+    topk(prob[keep].flatten(), min(max_num_inst, K*C)); boxes -> xyxy, Boxes.scale(w, h)
+
+which synchronises with the host once per class and again for the NMS result.  ``postprocess_detections`` computes the
+same outputs without a host round trip, so it can be captured into a CUDA graph with the rest of a frame.
+"""
+from __future__ import annotations
+
+import ctypes
+import functools
+from typing import Dict, NamedTuple, Optional, Sequence, Tuple, Union
+
+import torch
+
+from uninext_b200 import _cabi
+
+MAX_QUERIES, MAX_TOKENS, MAX_CLASSES = 1024, 256, 4096      # include/msda_b200.h
+LAUNCHES = 2                                                  # per call, whatever B, Q, C and nms_iou
+
+
+class Detections(NamedTuple):
+    """``[B, max_num_inst]`` each (``boxes`` ``[B, max_num_inst, 4]``), ``count`` ``[B]``.  Entries at and past
+    ``count[b]`` hold the fill values: score 0, label -1, query_index -1, box 0."""
+    scores: torch.Tensor          # fp32, descending per image
+    labels: torch.Tensor          # int32 class index c, 0-based (the reference's pred_classes)
+    boxes: torch.Tensor           # fp32 xyxy in pixels of the image size (Boxes.scale(w, h))
+    query_index: torch.Tensor     # int32 index into the Q queries: gathers the matching mask logits
+    count: torch.Tensor           # int32 valid entries per image, min(max_num_inst, K*C)
+
+
+@functools.lru_cache(maxsize=64)
+def _csr(items: Tuple[Tuple[int, Tuple[int, ...]], ...], device: torch.device) -> Tuple[torch.Tensor, torch.Tensor]:
+    """positive map content -> (class_start [C + 1], tokens [nnz]) int32 on the device.  Cached per
+    distinct content: one small host-to-device copy the first time, none afterwards (nor inside a graph capture)."""
+    starts, toks = [0], []
+    for _, t in items:
+        toks.extend(t)
+        starts.append(len(toks))
+    return torch.tensor(starts, dtype=torch.int32, device=device), torch.tensor(toks, dtype=torch.int32, device=device)
+
+
+# Cached device tensors that a captured CUDA graph reads: never freed, whatever the LRU caches above drop.
+_CAPTURED: Dict[int, torch.Tensor] = {}
+
+
+@functools.lru_cache(maxsize=256)
+def _sizes(sizes: Tuple[Tuple[int, int], ...], device: torch.device) -> torch.Tensor:
+    return torch.tensor(sizes, dtype=torch.int32, device=device)
+
+
+def positive_map_to_csr(positive_map: Dict[int, Sequence[int]], num_tokens: int,
+                        device: Union[str, torch.device] = "cuda") -> Tuple[torch.Tensor, torch.Tensor]:
+    """The reference's ``positive_map_label_to_token`` ({label: [token, ...]}, labels 1..C) as CSR on ``device``: class c
+    (= label - 1) owns ``tokens[class_start[c]:class_start[c + 1]]``, in the listed order.  Raises ValueError for labels
+    that are not exactly 1..C (the reference raises IndexError or leaves zero columns), for an empty token list (the
+    reference's mean is NaN) and for a token outside [0, num_tokens)."""
+    labels = sorted(int(k) for k in positive_map)
+    if not labels or labels != list(range(1, len(labels) + 1)):
+        raise ValueError(f"positive_map: labels must be exactly 1..C, got {labels[:8]}{'...' if len(labels) > 8 else ''}")
+    items = tuple((k, tuple(int(t) for t in positive_map[k])) for k in labels)
+    for k, t in items:
+        if not t:
+            raise ValueError(f"positive_map: label {k} has no tokens")
+        if min(t) < 0 or max(t) >= num_tokens:
+            raise ValueError(f"positive_map: label {k} has a token outside [0, {num_tokens}): {list(t)}")
+    if len(items) > MAX_CLASSES:
+        raise ValueError(f"positive_map: at most {MAX_CLASSES} classes, got {len(items)}")
+    return _csr(items, torch.device(device))
+
+
+def postprocess_detections(box_cls: torch.Tensor, box_pred: torch.Tensor, positive_map: Dict[int, Sequence[int]],
+                           image_sizes: Union[Sequence[Sequence[int]], torch.Tensor], iou_pred: Optional[torch.Tensor] = None,
+                           nms_iou: Optional[float] = 0.7, max_num_inst: int = 100) -> Detections:
+    """box_cls [B, Q, T] token logits, box_pred [B, Q, 4] normalised cxcywh, iou_pred [B, Q, 1] / [B, Q] or None,
+    positive_map = the reference's ``positive_map_label_to_token``, image_sizes = B pairs (h, w) or an int32 CUDA tensor
+    [B, 2].  ``nms_iou=None`` is the reference's OTA-off branch (no NMS); ``max_num_inst`` is 100 for detection, 1 for
+    grounding and SOT.  Q <= 1024, T <= 256, C <= 4096, 1 <= max_num_inst <= Q*C.
+
+    The result equals the reference chain's scores, pred_classes, pred_boxes and the query each came from, in its order.
+    One deliberate difference: ``uninext_vid.py``'s copy calls ``topk(100)`` without ``min`` and raises when K*C < 100;
+    here ``count`` is then below 100, as in ``uninext_img.py``.  Non-fp32 inputs are cast with ``.float()``.
+
+    Reference call sites (``projects/UNINEXT/uninext/``), with ``nms = 0.7 if self.ota else None``:
+      * ``uninext_img.py:284`` (detection / grounding): ``postprocess_detections(box_cls, box_pred, positive_map,
+        image_sizes, iou_pred, nms, 100 if task == "detection" else 1)``; the masks follow with
+        ``n = int(d.count[b]); paste_masks(mask_pred[b][d.query_index[b, :n]], image_size, output_size, 4, self.mask_thres)``.
+      * ``uninext_vid.py:511`` (SOT), ``:751`` (``inference_ytbvos``) and ``:889`` (``inference_ytbvos_3f``): all three
+        are reached only from ``task == "sot"`` with the map ``{1: [0]}``, so ``max_num_inst=1``:
+        ``postprocess_detections(box_cls, box_pred, {1: [0]}, image_sizes, iou_pred, nms, 1)``.  The two VOS sites pass
+        ``binary_mask=False``: their masks are the probabilities cropped to the image, ``paste_masks(mask_pred[b][
+        d.query_index[b, :1]], image_size, image_size, 4, threshold=None)``.
+
+    The positive map and the image sizes become small device tensors, cached per distinct content.  Those used while a
+    CUDA graph is being captured are kept for the life of the process, so the graph's replays never read freed memory
+    even after the cache has dropped them.
+    """
+    if not (box_cls.is_cuda and box_pred.is_cuda and (iou_pred is None or iou_pred.is_cuda)):
+        raise RuntimeError("postprocess_detections: Not implemented on the CPU")
+    if box_cls.dim() != 3 or box_pred.shape != (*box_cls.shape[:2], 4):
+        raise ValueError(f"postprocess_detections: need box_cls [B, Q, T] and box_pred [B, Q, 4], got "
+                         f"{tuple(box_cls.shape)} and {tuple(box_pred.shape)}")
+    b, q, t = box_cls.shape
+    dev = box_cls.device
+    if iou_pred is not None:
+        if iou_pred.shape not in ((b, q, 1), (b, q)):
+            raise ValueError(f"postprocess_detections: iou_pred must be [B, Q, 1] or [B, Q], got {tuple(iou_pred.shape)}")
+        iou_pred = iou_pred.float().contiguous()
+    if not (1 <= q <= MAX_QUERIES and 1 <= t <= MAX_TOKENS):
+        raise ValueError(f"postprocess_detections: need 1 <= Q <= {MAX_QUERIES} and 1 <= T <= {MAX_TOKENS}, got Q={q}, T={t}")
+    class_start, tokens = positive_map_to_csr(positive_map, t, dev)
+    c = class_start.numel() - 1
+    k = int(max_num_inst)
+    if not 1 <= k <= q * c:
+        raise ValueError(f"postprocess_detections: need 1 <= max_num_inst <= Q*C = {q * c}, got {k}")
+    if isinstance(image_sizes, torch.Tensor):
+        if not image_sizes.is_cuda or image_sizes.shape != (b, 2):
+            raise ValueError("postprocess_detections: an image_sizes tensor must be a CUDA tensor [B, 2] (h, w)")
+        sizes = image_sizes.to(torch.int32).contiguous()
+    else:
+        sizes = _sizes(tuple((int(s[0]), int(s[1])) for s in image_sizes), dev)
+        if sizes.shape != (b, 2):
+            raise ValueError(f"postprocess_detections: {b} images but {sizes.shape[0]} image sizes")
+    if torch.cuda.is_current_stream_capturing():
+        for held in (class_start, tokens, sizes):
+            _CAPTURED[id(held)] = held
+    x = box_cls.float().contiguous()
+    bx = box_pred.float().contiguous()
+    lib = _cabi.load()
+    ws_bytes = ctypes.c_int64(0)
+    _cabi.check(lib.msda_detpost_workspace(b, q, t, c, k, ctypes.byref(ws_bytes)), "msda_detpost_workspace")
+    out = Detections(torch.empty((b, k), dtype=torch.float32, device=dev), torch.empty((b, k), dtype=torch.int32, device=dev),
+                     torch.empty((b, k, 4), dtype=torch.float32, device=dev),
+                     torch.empty((b, k), dtype=torch.int32, device=dev), torch.empty((b,), dtype=torch.int32, device=dev))
+    ws = torch.empty(max(int(ws_bytes.value), 16), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _cabi.check(lib.msda_detpost_f32(x.data_ptr(), bx.data_ptr(), iou_pred.data_ptr() if iou_pred is not None else None,
+                                         class_start.data_ptr(), tokens.data_ptr(), sizes.data_ptr(), b, q, t, c,
+                                         int(nms_iou is not None), float(nms_iou) if nms_iou is not None else 0.0, k,
+                                         out.scores.data_ptr(), out.labels.data_ptr(), out.query_index.data_ptr(),
+                                         out.boxes.data_ptr(), out.count.data_ptr(), ws.data_ptr(), ws.numel(),
+                                         torch.cuda.current_stream().cuda_stream), "msda_detpost_f32")
+    return out
+
