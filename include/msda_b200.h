@@ -45,8 +45,8 @@
 extern "C" {
 #endif
 
-#define MSDA_ABI_VERSION 10  /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
-                                8: msda_vlfuse_*_bf16; 9: msda_mask_paste_f32; 10: msda_detpost_* */
+#define MSDA_ABI_VERSION 11  /* 4: MSDA_KNOB_REGION_BWD; 5: msda_backward_det_*; 6: msda_vlfuse_*; 7: msda_vlfuse_*_tf32;
+                                8: msda_vlfuse_*_bf16; 9: msda_mask_paste_f32; 10: msda_detpost_*; 11: msda_mask_rle_* */
 
 #define MSDA_E_BADARG   (-1)   /* null pointer, non-positive dimension, unknown knob                  */
 #define MSDA_E_TOOLARGE (-2)   /* a dimension product exceeds what the kernels index (see msda_b200.h) */
@@ -298,6 +298,40 @@ int msda_detpost_f32(const float *box_cls, const float *box_pred, const float *i
                      const int *tokens, const int *image_sizes, int B, int Q, int T, int C, int nms, float nms_iou,
                      int max_num_inst, float *scores, int *labels, int *query_index, float *boxes, int *count,
                      void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---- COCO run-length encoding of masks for inference (DESIGN.md section 3.14, row f-7; uninext_vid.py:1425-1432,
+ * :1263-1271 + :1686-1700, detectron2/evaluation/coco_evaluation.py:478-490) ---------------------------------------------
+ * The `counts` strings of pycocotools' mask.encode, for I masks of out_h x out_w pixels:
+ *   bits    msda_mask_rle_count_f32: bit (Y, X) of instance i is the pixel msda_mask_paste_f32 writes with binary != 0
+ *           for the same arguments (steps 1-4 of section 3.12, p > threshold), evaluated by the same device code;
+ *           msda_mask_rle_count_u8: masks [I, out_h, out_w] uint8 / bool, row-major, any alignment; the bit is mask != 0.
+ *   counts  (rleEncode) scan column-major, k = X * out_h + Y; boundaries are the k with bit(k) != bit(k - 1), bit(-1) = 0;
+ *           the counts are the differences of 0, the boundaries and out_h * out_w (counts[0] = 0 when pixel 0 is set).
+ *   string  (rleToString) x = counts[j] - counts[j - 2] for j > 2, counts[j] otherwise; x is written as 5-bit groups,
+ *           least significant first: c = x & 0x1f, x >>= 5 (arithmetic), continue while (c & 0x10 ? x != -1 : x != 0);
+ *           0x20 is set on every character of a value but its last, and 48 is added.  At most 7 characters per count.
+ * A call is two steps with one host read between them:
+ *   1. msda_mask_rle_count_*: pass 1 (the bitmap and every column's boundary count) and an in-place scan.  On return the
+ *      workspace begins with int64 [I * out_w + 1]: entry i * out_w is the number of boundaries before instance i, entry
+ *      I * out_w the total B.  3 launches.
+ *   2. the caller reads B, then msda_mask_rle_encode with `boundaries` = B, positions uint32 [B] (NULL allowed when B = 0),
+ *      chars of at least 7 * (B + I) bytes and byte_offsets int64 [I + 1].  It writes instance i's string to
+ *      chars[byte_offsets[i] .. byte_offsets[i + 1]), the strings back to back from byte_offsets[0] = 0.  4 launches.
+ * msda_mask_rle_workspace: the workspace bytes for (I, out_h, out_w): the column offsets, the bitmap [I][ceil(out_h / 32)]
+ *   [out_w] uint32, the scan's storage and one int64 per 2048 possible counts; 0 for I = 0.
+ * Limits: I >= 0 (0: no launch), out_h, out_w >= 1, non-null pointers, a 16-byte aligned workspace of at least
+ * msda_mask_rle_workspace bytes, 0 <= boundaries <= I * out_h * out_w; otherwise MSDA_E_BADARG.  MSDA_E_TOOLARGE if
+ * out_h * out_w > 2^32 - 1 (the COCO API's counts are 32-bit unsigned), out_w >= 2^30 or I >= 2^31; the logits entry also
+ * has msda_mask_paste_f32's limits.  Offsets are 64-bit.  Nothing is allocated; the host must read B between the steps,
+ * so a call cannot be captured into a CUDA graph. */
+int msda_mask_rle_workspace(int64_t I, int out_h, int out_w, int64_t *bytes);
+int msda_mask_rle_count_f32(const float *logits, int64_t I, int Hs, int Ws, int stride, int crop_h, int crop_w,
+                            int out_h, int out_w, float threshold, void *workspace, int64_t workspace_bytes,
+                            void *stream);
+int msda_mask_rle_count_u8(const uint8_t *masks, int64_t I, int out_h, int out_w, void *workspace,
+                           int64_t workspace_bytes, void *stream);
+int msda_mask_rle_encode(int64_t I, int out_h, int out_w, int64_t boundaries, void *workspace, int64_t workspace_bytes,
+                         uint32_t *positions, int64_t *byte_offsets, char *chars, void *stream);
 
 /* ---- TF32 GEMM for the Linears that bracket the op:  C[M,N] = A[M,K] . W[N,K]^T + bias[N]  (fp32 storage, sm_90 wgmma TF32
  * MMA with fp32 accumulation; TMA-fed).  K % 32 == 0, N % 32 == 0 (N % 64 == 0 above 256), N <= 512.

@@ -51,6 +51,10 @@ SIGNATURES = {
     "msda_aligned_bilinear_forward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
     "msda_aligned_bilinear_backward_f32": (_i, [_vp, ctypes.c_int64, _i, _i, _i, _vp, _vp]),
     "msda_mask_paste_f32": (_i, [_vp, ctypes.c_int64] + [_i] * 7 + [ctypes.c_float, _i, _vp, _vp]),
+    "msda_mask_rle_workspace": (_i, [ctypes.c_int64, _i, _i, _vp]),
+    "msda_mask_rle_count_f32": (_i, [_vp, ctypes.c_int64] + [_i] * 7 + [ctypes.c_float, _vp, ctypes.c_int64, _vp]),
+    "msda_mask_rle_count_u8": (_i, [_vp, ctypes.c_int64, _i, _i, _vp, ctypes.c_int64, _vp]),
+    "msda_mask_rle_encode": (_i, [ctypes.c_int64, _i, _i, ctypes.c_int64, _vp, ctypes.c_int64] + [_vp] * 4),
     "msda_detpost_workspace": (_i, [_i] * 5 + [_vp]),
     "msda_detpost_f32": (_i, [_vp] * 6 + [_i] * 5 + [ctypes.c_float, _i] + [_vp] * 6 + [ctypes.c_int64, _vp]),
     "msda_vlfuse_workspace": (_i, [_i] * 5 + [_vp]),
@@ -62,7 +66,7 @@ SIGNATURES = {
     "msda_vlfuse_forward_bf16": (_i, [_vp] * 5 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 4 + [ctypes.c_int64, _vp]),
     "msda_vlfuse_backward_bf16": (_i, [_vp] * 10 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 5 + [ctypes.c_int64, _vp]),
 }
-ABI_VERSION = 10
+ABI_VERSION = 11
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 

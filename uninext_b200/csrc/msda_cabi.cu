@@ -11,6 +11,7 @@
 #include "msda_detpost.cuh"
 #include "msda_generic.cuh"
 #include "msda_maskpaste.cuh"
+#include "msda_maskrle.cuh"
 #include "msda_module.cuh"
 #include "msda_region.cuh"
 #include "msda_slab.cuh"
@@ -1169,6 +1170,139 @@ int msda_detpost_f32(const float *box_cls, const float *box_pred, const float *i
                                                                     labels, query_index, boxes, count);
     }
     g_launches.fetch_add(2, std::memory_order_relaxed);
+    return (int)cudaGetLastError();
+}
+
+}  // extern "C"
+
+// ---- COCO run-length encoding of masks (f-7) ----------------------------------------------------------------------------
+namespace {
+
+struct RleLayout {
+    size_t col_off, bitmap, scan, scan_bytes, tiles, total;
+};
+
+int rle_check(long long I, int out_h, int out_w) {
+    if (I < 0 || out_h < 1 || out_w < 1) return MSDA_E_BADARG;
+    // The COCO API's counts are 32-bit unsigned: a mask of more than 2^32 - 1 pixels has no RLE.
+    if (I >= (1ll << 31) || (unsigned long long)out_h * (unsigned)out_w > 0xffffffffull || out_w >= (1 << 30))
+        return MSDA_E_TOOLARGE;
+    return 0;
+}
+
+// [I * W + 1] column offsets (first, so the caller finds the total at entry I * W), the bitmap, cub's scan storage and
+// pass 3's tile sums for the most counts an instance can have (every pixel a boundary, plus one).
+int rle_layout(long long I, int out_h, int out_w, RleLayout &l) {
+    const long long cols = I * out_w + 1, nw = (out_h + 31) / 32;
+    const long long max_tiles = (I * ((long long)out_h * out_w + 1) + msda::kRleTile - 1) / msda::kRleTile;
+    l.scan_bytes = 0;
+    const cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, l.scan_bytes, (long long *)nullptr, cols);
+    if (e != cudaSuccess) return (int)e;
+    l.col_off = 0;
+    l.bitmap = dp_align(l.col_off + (size_t)cols * sizeof(long long));
+    l.scan = dp_align(l.bitmap + (size_t)I * nw * out_w * sizeof(unsigned));
+    l.tiles = dp_align(l.scan + l.scan_bytes);
+    l.total = dp_align(l.tiles + (size_t)max_tiles * sizeof(long long));
+    return 0;
+}
+
+dim3 rle_grid(long long I, int out_w, int cols_per_thread) {
+    const long long per_block = (long long)msda::kRleThreads * cols_per_thread;
+    return dim3((unsigned)((out_w + per_block - 1) / per_block), (unsigned)(I < 65535 ? I : 65535));
+}
+
+// The scan after pass 1 (cub: an init kernel and the scan kernel); counts pass 1 and the scan's two launches.
+int rle_scan(long long I, int out_w, const RleLayout &l, char *ws, cudaStream_t st) {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return (int)e;
+    size_t scan_bytes = l.scan_bytes;
+    e = cub::DeviceScan::ExclusiveSum(ws + l.scan, scan_bytes, reinterpret_cast<long long *>(ws + l.col_off),
+                                      I * out_w + 1, st);
+    g_launches.fetch_add(3, std::memory_order_relaxed);
+    return e != cudaSuccess ? (int)e : (int)cudaGetLastError();
+}
+
+}  // namespace
+
+extern "C" {
+
+int msda_mask_rle_workspace(int64_t I, int out_h, int out_w, int64_t *bytes) {
+    if (!bytes) return MSDA_E_BADARG;
+    if (const int c = rle_check(I, out_h, out_w)) return c;
+    if (I == 0) { *bytes = 0; return 0; }
+    RleLayout l;
+    if (const int e = rle_layout(I, out_h, out_w, l)) return e;
+    *bytes = (int64_t)l.total;
+    return 0;
+}
+
+int msda_mask_rle_count_f32(const float *logits, int64_t I, int Hs, int Ws, int stride, int crop_h, int crop_w,
+                            int out_h, int out_w, float threshold, void *workspace, int64_t workspace_bytes,
+                            void *stream) {
+    if (!logits || !workspace || !aligned16(workspace) || I < 0 || Hs <= 0 || Ws <= 0 || stride <= 0 || crop_h <= 0 ||
+        crop_w <= 0 || out_h <= 0 || out_w <= 0 || (long long)stride * Hs >= (1ll << 31) ||
+        (long long)stride * Ws >= (1ll << 31) || crop_h > stride * Hs || crop_w > stride * Ws)
+        return MSDA_E_BADARG;
+    if (out_h > 65535 * msda::kMpRows) return MSDA_E_TOOLARGE;           // msda_mask_paste_f32's limits
+    if (const int c = rle_check(I, out_h, out_w)) return c;
+    if (I == 0) return 0;
+    RleLayout l;
+    if (const int e = rle_layout(I, out_h, out_w, l)) return e;
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // The scales exactly as msda_mask_paste_f32 forms them.
+    const float near_y = (float)crop_h / (float)out_h, near_x = (float)crop_w / (float)out_w;
+    const float lin_y = (float)Hs / (float)(stride * Hs), lin_x = (float)Ws / (float)(stride * Ws);
+    msda::rle_bits_logits<<<rle_grid(I, out_w, 1), msda::kRleThreads, 0, st>>>(
+        logits, I, Hs, Ws, crop_h, crop_w, out_h, out_w, near_y, near_x, lin_y, lin_x, threshold,
+        reinterpret_cast<unsigned *>(ws + l.bitmap), reinterpret_cast<long long *>(ws + l.col_off));
+    return rle_scan(I, out_w, l, ws, st);
+}
+
+int msda_mask_rle_count_u8(const uint8_t *masks, int64_t I, int out_h, int out_w, void *workspace,
+                           int64_t workspace_bytes, void *stream) {
+    if (!masks || !workspace || !aligned16(workspace)) return MSDA_E_BADARG;
+    if (const int c = rle_check(I, out_h, out_w)) return c;
+    if (I == 0) return 0;
+    RleLayout l;
+    if (const int e = rle_layout(I, out_h, out_w, l)) return e;
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    unsigned *bitmap = reinterpret_cast<unsigned *>(ws + l.bitmap);
+    long long *col_count = reinterpret_cast<long long *>(ws + l.col_off);
+    const dim3 grid = rle_grid(I, out_w, msda::kRleU8Cols);
+    if ((reinterpret_cast<uintptr_t>(masks) & 3u) == 0 && out_w % 4 == 0)
+        msda::rle_bits_u8<true><<<grid, msda::kRleThreads, 0, st>>>(masks, I, out_h, out_w, bitmap, col_count);
+    else
+        msda::rle_bits_u8<false><<<grid, msda::kRleThreads, 0, st>>>(masks, I, out_h, out_w, bitmap, col_count);
+    return rle_scan(I, out_w, l, ws, st);
+}
+
+int msda_mask_rle_encode(int64_t I, int out_h, int out_w, int64_t boundaries, void *workspace, int64_t workspace_bytes,
+                         uint32_t *positions, int64_t *byte_offsets, char *chars, void *stream) {
+    if (!workspace || !aligned16(workspace) || !byte_offsets || !chars || (boundaries > 0 && !positions) ||
+        (reinterpret_cast<uintptr_t>(positions) & 3u) || (reinterpret_cast<uintptr_t>(byte_offsets) & 7u))
+        return MSDA_E_BADARG;
+    if (const int c = rle_check(I, out_h, out_w)) return c;
+    if (boundaries < 0 || (I > 0 && boundaries > I * ((long long)out_h * out_w))) return MSDA_E_BADARG;
+    if (I == 0) return 0;
+    RleLayout l;
+    if (const int e = rle_layout(I, out_h, out_w, l)) return e;
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    char *ws = static_cast<char *>(workspace);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long *col_off = reinterpret_cast<const long long *>(ws + l.col_off);
+    long long *tiles = reinterpret_cast<long long *>(ws + l.tiles);
+    msda::rle_boundaries<<<rle_grid(I, out_w, 1), msda::kRleThreads, 0, st>>>(
+        reinterpret_cast<const unsigned *>(ws + l.bitmap), col_off, I, out_h, out_w, positions);
+    const msda::RleCounts rc{col_off, positions, I, boundaries + I, (long long)out_h * out_w, out_w};
+    const long long ntiles = (rc.N + msda::kRleTile - 1) / msda::kRleTile;
+    msda::rle_tile_bytes<<<(unsigned)ntiles, msda::kRleTileThreads, 0, st>>>(rc, tiles);
+    msda::rle_scan_tiles<<<1, msda::kRleScanThreads, 0, st>>>(tiles, ntiles);
+    msda::rle_write<<<(unsigned)ntiles, msda::kRleTileThreads, 0, st>>>(rc, tiles, reinterpret_cast<long long *>(byte_offsets), chars);
+    g_launches.fetch_add(4, std::memory_order_relaxed);
     return (int)cudaGetLastError();
 }
 

@@ -38,6 +38,15 @@ __device__ __forceinline__ void mp_source(int o, float near_scale, int crop, flo
     l1 = src - (float)i0;
 }
 
+// The probability at one output pixel: upsample_bilinear2d's expression and order over the taps t0[0], t0[dx], t1[0],
+// t1[dx] (t0, t1 = the source rows at the pixel's first tap column, hy0 = 1 - ly), then torch's fp32 sigmoid.  mask_paste
+// and the RLE pass (msda_maskrle.cuh) both evaluate pixels through this, so their bits cannot differ.
+__device__ __forceinline__ float mp_prob(const float *t0, const float *t1, int dx, float lx, float hy0, float ly) {
+    const float w0 = 1.f - lx;
+    const float v = hy0 * (w0 * __ldg(t0) + lx * __ldg(t0 + dx)) + ly * (w0 * __ldg(t1) + lx * __ldg(t1 + dx));
+    return 1.f / (1.f + expf(-v));
+}
+
 // block: (kMpGroups, kMpRows); grid: (column tiles, row tiles, instance chunks of kMpInst; grid-z strides over I).
 // out: uint8 [I, out_h, out_w] (BINARY) or fp32.  VEC: out is 16-byte aligned and out_w is a multiple of the store
 // vector (8 bytes / 4 floats), so a vector is either wholly inside a row or wholly past its end.
@@ -74,13 +83,7 @@ mask_paste(const float *__restrict__ logits, long long I, int Hs, int Ws, int cr
             const float *r0 = base + (size_t)y0 * Ws, *r1 = base + (size_t)y1 * Ws;
             float p[kMpCols];
 #pragma unroll
-            for (int k = 0; k < kMpCols; ++k) {
-                // upsample_bilinear2d's expression and order, then torch's fp32 sigmoid
-                const float w0 = 1.f - lx[k];
-                const float v = hy0 * (w0 * __ldg(r0 + x0[k]) + lx[k] * __ldg(r0 + x0[k] + dx[k])) +
-                                ly * (w0 * __ldg(r1 + x0[k]) + lx[k] * __ldg(r1 + x0[k] + dx[k]));
-                p[k] = 1.f / (1.f + expf(-v));
-            }
+            for (int k = 0; k < kMpCols; ++k) p[k] = mp_prob(r0 + x0[k], r1 + x0[k], dx[k], lx[k], hy0, ly);
             const size_t o = (size_t)i * out_plane + out_row;
             if constexpr (BINARY) {
                 uint8_t *dst = static_cast<uint8_t *>(out) + o;
