@@ -1,6 +1,7 @@
 // Driver for tools/region_phases.py: msda_bwd_region<8, HALO> built with the phase-clock hook (MSDA_REGION_PHASE_CLOCKS,
 // msda_region.cuh) for HALO in 1..6, launched as the library launches it (region_smem_bytes() of dynamic shared memory,
-// occupancy x SMs CTAs).  Plain C entry points for ctypes; the caller zero-fills grad_value and owns the clock buffer.
+// occupancy x SMs CTAs, TMA-staged taps when L*P % 4 == 0).  Plain C entry points for ctypes; the caller zero-fills
+// grad_value and owns the clock buffer ([grid x kRegionSpans] u64).
 #define MSDA_REGION_PHASE_CLOCKS
 #include "msda_region.cuh"
 
@@ -25,13 +26,14 @@ int launch(int setup, unsigned long long *clocks, int knockout, const float *go,
         return grid;
     }
     const unsigned npairs = (unsigned)((long long)N * Lq * M);
-    kern<<<grid, msda::kTiledThreads, smem>>>(go, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, gv, gl, ga);
+    const int tma = (L * P) % 4 == 0 ? 1 : 0;
+    kern<<<grid, msda::kTiledThreads, smem>>>(go, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, tma, gv, gl, ga);
     return cudaGetLastError() == cudaSuccess ? grid : -1;
 }
 
 }  // namespace
 
-// setup != 0: point the hook at `clocks` ([grid x 4] u64) and set the knockout bits; returns the grid size (-1 on error).
+// setup != 0: point the hook at `clocks` ([grid x kRegionSpans] u64) and set the knockout bits; returns the grid size (-1 on error).
 // setup == 0: one launch on the legacy default stream; returns the grid size (-1 on error).
 extern "C" int region_phases_run(int halo, int setup, unsigned long long *clocks, int knockout, const float *go,
                                  const float *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
@@ -47,3 +49,5 @@ extern "C" int region_phases_run(int halo, int setup, unsigned long long *clocks
     }
     return -1;
 }
+
+extern "C" int region_phases_spans() { return msda::kRegionSpans; }

@@ -6,13 +6,14 @@ cfg2 encoder input (seed 1000), for each halo of a sweep.
 
 Compiles tools/region_phases.cu -- the kernel header with the MSDA_REGION_PHASE_CLOCKS hook, msda_bwd_region<8, HALO>
 for HALO in 1..6 -- with nvcc for sm_90a into a temporary directory, and launches it as the library does.  Thread 0 of
-each CTA sums clock64() spans taken after CTA barriers: prologue + tile geometry + staging, phase A (gathers, entries,
-direct reds), phase B (sort), phase C (row sums, one red per touched row).  Prints, per halo:
+each CTA sums clock64() spans taken after CTA barriers: the tap pass (gathers, grad_loc / grad_attn), tile geometry and
+count reset, phase A (tap geometry, entries, direct reds), phase B (sort), phase C (row sums, one red per touched row).
+Prints, per halo:
   - the hooked kernel's time (CUDA events, median of `iters` launches; no zero-fill, no L2 flush);
   - each span's share of its CTA's cycles, median over CTAs, and that share of the kernel time;
   - the knockout times: no phase-A reds, no phase-C reds, neither (results wrong by construction: timing only);
-and the GPU's name and power limit.  --csrc points the driver at another copy of the kernel headers (e.g. an older
-version with the same hook) for before / after tables."""
+and the GPU's name and power limit.  --csrc points the driver at another copy of the kernel headers with the same hook
+and launch signature, for before / after tables."""
 import argparse
 import ctypes
 import os
@@ -29,7 +30,7 @@ sys.path.insert(0, ROOT)
 from uninext_b200 import build as libbuild  # noqa: E402
 from uninext_b200.workloads import CONFIGS, make_inputs  # noqa: E402
 
-SPANS = ("prologue+staging", "phase A", "phase B", "phase C")
+SPANS = ("tap pass", "tile geometry", "phase A", "phase B", "phase C")
 KNOCKOUTS = ((1, "no phase-A reds"), (2, "no phase-C reds"), (3, "no reds at all"))
 
 
@@ -72,6 +73,8 @@ def main():
         lib = ctypes.CDLL(compile_driver(os.path.abspath(args.csrc), tmp))
     finally:
         shutil.rmtree(tmp, ignore_errors=True)      # the loaded library stays mapped
+    nspans = lib.region_phases_spans()
+    assert nspans == len(SPANS), (nspans, SPANS)
     fn = lib.region_phases_run
     fn.restype = ctypes.c_int
     fn.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 6 + \
@@ -109,12 +112,12 @@ def main():
           f"phase-clock hook, median of {args.iters} launches; csrc {os.path.relpath(os.path.abspath(args.csrc), ROOT)}")
     for halo in halos:
         grid = fn(halo, 1, 0, 0, *ptrs, *dims, *outs)
-        clocks = torch.zeros(grid * 4, dtype=torch.int64, device="cuda")
+        clocks = torch.zeros(grid * nspans, dtype=torch.int64, device="cuda")
         ms = run(halo, 0, clocks)
-        c = clocks.view(grid, 4).double().cpu()
+        c = clocks.view(grid, nspans).double().cpu()
         c = c[c.sum(1) > 0]
         shares = c / c.sum(1, keepdim=True)
-        med = [float(shares[:, k].median()) for k in range(4)]
+        med = [float(shares[:, k].median()) for k in range(nspans)]
         print(f"--- halo {halo}: {ms:.4f} ms ({grid} CTAs)")
         for k, name in enumerate(SPANS):
             print(f"  {name:17s} {100 * med[k]:5.1f} %  ~{med[k] * ms:.4f} ms")

@@ -413,8 +413,9 @@ cudaError_t launch_bwd_region(const float *go, const float *value, const int64_t
         slots_c[dev].store(slots, std::memory_order_relaxed);
     }
     const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
+    const int tma = use_tma_staging(d) ? 1 : 0;            // the tap pass: TMA-staged or __ldg taps, as msda_bwd_tiled
     const cudaError_t e = launch_after_fill(kern, slots, smem, st, go, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq,
-                                            d.P, npairs, gv, gl, ga);
+                                            d.P, npairs, tma, gv, gl, ga);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return e;
 }

@@ -7,23 +7,24 @@
 // queries of one (batch, head) whose pixel centre lies in one R x R region of the finest level touches only a small
 // rectangle ("window") of each level, and it can add those contributions up on chip first.
 //
-// Tile = (b, m, region).  A query at pixel (x, y) of level l belongs to region floor((x + 0.5) * Wref / W_l / R) in x (likewise
-// in y; Wref / Href = the largest level), so a region holds one contiguous x-range and y-range per level, in closed form.
-// The window on level l is the region scaled to level l plus kRegionHalo pixels.  Per tile:
-//   staging: the value rows of the window's last levels (the coarsest of a feature pyramid, whose rows are gathered most
-//            often) are copied into shared memory with 16-byte cp.async, from the last level down while they fit
-//            kRegionStageRows.  The staged rows are a suffix [sfirst, nwin) of the window-row numbering.
-//   phase A (one 8-lane group per pair, as msda_bwd_tiled): gathers, grad_loc / grad_attn epilogue unchanged; a corner
-//            inside a staged level is read from shared memory, every other corner from global memory (same values, same
-//            FMA order).  The pair's grad_out row is stashed in shared memory; a non-zero corner inside the window
-//            becomes an entry {window row, coefficient} at the fixed position (slot, tap, corner), and the filing lane
-//            counts it for its window row with a non-returning shared atomic (nothing on the gather path waits for it).
-//            A corner outside the window, or of a query past the stash, reds directly as in msda_bwd_tiled, so the
-//            capacities never change a result.
-//   phase B: scan of the row counts, then scatter of the entries by window row (integer shared atomics only: fp32 shared
-//            atomics are CAS loops) into {coefficient, slot} arrays, which overlay the staged rows (dead after phase A).
-//   phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
-// A level table that does not tile [0, S) (the patch-order condition) runs in linear chunks of pairs with no window.
+// grad_value's sums need each tap's geometry and the pair's grad_out, never `value`.  So one launch runs two passes in
+// every CTA, one after the other:
+//   tap pass: msda_bwd_tiled's NORED body (linear chunks of pairs, taps TMA-staged one iteration ahead when L*P % 4 == 0):
+//             the gathers, grad_loc and grad_attn, from the same device code and in the same FMA order as msda_bwd_tiled.
+//   grad_value pass, per tile = (b, m, region).  A query at pixel (x, y) of level l belongs to region
+//             floor((x + 0.5) * Wref / W_l / R) in x (likewise in y; Wref / Href = the largest level), so a region holds
+//             one contiguous x-range and y-range per level, in closed form.  The window on level l is the region scaled to
+//             level l plus kRegionHalo pixels.
+//     phase A: one 8-lane group per pair; the lane that resolves a tap files its non-zero in-window corners as entries
+//              {window row, coefficient} at the fixed positions (slot, tap, corner) and counts each for its window row with
+//              a non-returning shared atomic.  The pair's grad_out row is stashed in shared memory.  A corner outside the
+//              window, or of a query past the stash, reds directly as in msda_bwd_tiled (its weight and rows go through
+//              the group's tap slab), so the capacities never change a result.  No value row is read.
+//     phase B: scan of the row counts, then scatter of the entries by window row (integer shared atomics only: fp32 shared
+//              atomics are CAS loops) into {coefficient, slot} arrays.
+//     phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
+// A level table that does not tile [0, S) (the patch-order condition) runs the grad_value pass in linear chunks of pairs
+// with no window: every corner reds directly.
 #pragma once
 
 #include "msda_tiled.cuh"
@@ -34,31 +35,39 @@ constexpr int kRegionEdge = 8;            // region edge, in pixels of the fines
 constexpr int kRegionHalo = 2;            // window margin around the scaled region, in pixels of each level (swept 1-6)
 constexpr int kRegionSlots = 96;          // queries per tile whose grad_out row is stashed (the rest red directly)
 constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past this budget red directly)
-constexpr int kRegionStageRows = 384;     // window rows staged in shared memory (cfg2: every level, at most 274 rows)
+// Not used by the kernel, which stages no value rows: only the tests' restatement of the window layout
+// (tests/region_layout.py) reads it.
+constexpr int kRegionStageRows = 384;
 constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
 constexpr int kRegionMinCtas = 2;
 constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
 
-// entry coefficients (f32) + grad_out stash + row counts + entry rows (u16) + the larger of the staged value rows and
-// the sorted {coefficient (f32), slot (u8)} arrays, which share their space
+// The tap pass's TMA stage buffers (kTiledWarps per-warp double buffers of one iteration's (x, y, a)).
+using RegionTapStage = TapStage<4, 16, true>;
+
+// Dynamic shared memory: entry coefficients (f32) + grad_out stash + row counts + entry rows (u16) + the sorted
+// {coefficient (f32), slot (u8)} arrays.  The tap pass's stage buffers overlay the entry coefficients: the passes run
+// one after the other.
 constexpr size_t region_smem_bytes() {
-    constexpr size_t staged = (size_t)kRegionStageRows * 128, sorted = (size_t)kRegionEntries * (4 + 1);
+    static_assert((size_t)kTiledWarps * RegionTapStage::kBytes <= (size_t)kRegionEntries * 4, "stage buffers overlay e_coef");
     return (size_t)kRegionEntries * (4 + 2) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4 +
-           (staged > sorted ? staged : sorted);
+           (size_t)kRegionEntries * (4 + 1);
 }
 
 #ifdef MSDA_REGION_PHASE_CLOCKS
 // Timing hook for tools/region_phases.py; the library build never defines it.  Thread 0 of each CTA adds the clock64()
-// span since the previous stamp into g_region_clocks[blockIdx.x * 4 + span], after a CTA barrier: span 0 = prologue +
-// tile geometry + staging, 1 = phase A, 2 = phase B, 3 = phase C.  g_region_knockout bit 0 drops phase A's reds, bit 1
-// phase C's (the sums are still formed); results are then wrong by construction and serve only for timing.
+// span since the previous stamp into g_region_clocks[blockIdx.x * kRegionSpans + span], after a CTA barrier: span 0 = tap
+// pass, 1 = tile geometry + count reset, 2 = phase A, 3 = phase B, 4 = phase C.  g_region_knockout bit 0 drops phase A's
+// direct reds, bit 1 phase C's (the sums are still formed); results are then wrong by construction and serve only for
+// timing.
+constexpr int kRegionSpans = 5;
 __device__ unsigned long long *g_region_clocks;
 __device__ int g_region_knockout;
 #define MSDA_REGION_CLOCK_INIT long long region_clk = clock64()
 #define MSDA_REGION_CLOCK(span)                                                                  \
     if (threadIdx.x == 0) {                                                                      \
         const long long now = clock64();                                                         \
-        g_region_clocks[blockIdx.x * 4 + (span)] += (unsigned long long)(now - region_clk);      \
+        g_region_clocks[blockIdx.x * kRegionSpans + (span)] += (unsigned long long)(now - region_clk); \
         region_clk = now;                                                                        \
     }
 #define MSDA_REGION_KEEP_RED(bit) (!(g_region_knockout & (bit)))
@@ -67,11 +76,6 @@ __device__ int g_region_knockout;
 #define MSDA_REGION_CLOCK(span)
 #define MSDA_REGION_KEEP_RED(bit) true
 #endif
-
-__device__ __forceinline__ void cp_async16(void *dst, const void *src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 struct RegionMap {
     int H[kMaxLevels], W[kMaxLevels], start[kMaxLevels];
@@ -82,23 +86,9 @@ struct RegionMap {
 
 struct RegionTile {
     int b, m, nq, nwin;
-    int sfirst;                 // first staged window row: rows [sfirst, nwin) are in shared memory
     unsigned base_pair;         // linear chunks
     int qy0[kMaxLevels], qx0[kMaxLevels], qny[kMaxLevels], qnx[kMaxLevels], qpre[kMaxLevels + 1];
     int wy0[kMaxLevels], wx0[kMaxLevels], wh[kMaxLevels], ww[kMaxLevels], wbase[kMaxLevels + 1];
-};
-
-// Per-warp window records, laid out like TapSlab's row records:
-// {window row of corner 00, (dy * ww) << 6 | staged level << 5 | dw << 4 | in-window corner mask}.
-template <int LPR>
-struct WinSlab {
-    static constexpr int kStride = LPR * 8 + 8;
-    static constexpr int kBytes = (32 / LPR) * kStride;
-    int2 *p;
-    __device__ __forceinline__ WinSlab(unsigned char *warp_base, int grp)
-        : p(reinterpret_cast<int2 *>(warp_base + grp * kStride)) {}
-    __device__ __forceinline__ void put(int j, int2 v) { p[j] = v; }
-    __device__ __forceinline__ int2 get(int j) const { return p[j]; }
 };
 
 // First pixel of a level of n pixels (reference extent `ref`) whose region index is >= r.
@@ -107,13 +97,14 @@ __device__ __forceinline__ int region_first(int r, int n, int ref, int R) {
     return num <= 0 ? 0 : (int)min((long long)n, (num + 2ll * ref - 1) / (2ll * ref));
 }
 
+// The grad_value pass.  It is a separate function, called once per CTA, so that nothing it computes is hoisted into the
+// tap pass: the tap pass needs the kernel's whole 128-register budget (2 CTAs/SM), and any value of this pass kept live
+// through it is a spill.
 template <int R, int HALO>
-__global__ void __launch_bounds__(kTiledThreads, kRegionMinCtas)
-msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ value,
-                const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
-                const float *__restrict__ loc, const float *__restrict__ attn,
-                int N, int S, int M, int L, int Lq, int P, unsigned npairs,
-                float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn)
+__device__ __noinline__ void
+region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__restrict__ shapes,
+                       const int64_t *__restrict__ lsi, const float *__restrict__ loc, const float *__restrict__ attn,
+                       int N, int S, int M, int L, int Lq, int P, unsigned npairs, float *__restrict__ grad_value)
 {
     constexpr int D = 32, VEC = 4, LPR = D / VEC, GPW = 32 / LPR, LP_MAX = 16, NSL = LP_MAX / LPR;
     static_assert(GPW * kTiledWarps == kRegionIterSlots && kRegionSlots <= 256 && kRegionWinRows < 0xffff &&
@@ -124,24 +115,15 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
     __shared__ RegionTile tl;
     __shared__ int wsum[kTiledWarps];
     __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<LPR>::kBytes];
-    __shared__ __align__(16) unsigned char win_mem[kTiledWarps * WinSlab<LPR>::kBytes];
-    extern __shared__ __align__(16) unsigned char dyn[];
-    float *e_coef = reinterpret_cast<float *>(dyn);                                   // [slot][tap][corner]
+    extern __shared__ __align__(128) unsigned char region_dyn[];
+    float *e_coef = reinterpret_cast<float *>(region_dyn);                            // [slot][tap][corner]
     float4 *gstash = reinterpret_cast<float4 *>(e_coef + kRegionEntries);             // [slot][lane] grad_out slices
     int *cnt = reinterpret_cast<int *>(gstash + kRegionSlots * LPR);                  // [window row]
     unsigned short *e_row = reinterpret_cast<unsigned short *>(cnt + kRegionWinRows); // [slot][tap][corner], kNoRow = none
-    float4 *vstage = reinterpret_cast<float4 *>(e_row + kRegionEntries);              // phase A: [staged row][lane]
-    float *s_coef = reinterpret_cast<float *>(vstage);                                // phases B, C: sorted by window row
+    float *s_coef = reinterpret_cast<float *>(e_row + kRegionEntries);                // phases B, C: sorted by window row
     unsigned char *s_slot = reinterpret_cast<unsigned char *>(s_coef + kRegionEntries);
 
     MSDA_REGION_CLOCK_INIT;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int sub = lane % LPR, grp = lane / LPR;
-    const int LP = L * P;
-    const unsigned row_elems = (unsigned)(M * D);
-    TapSlab<LPR> slab(slab_mem + warp * TapSlab<LPR>::kBytes, grp);
-    WinSlab<LPR> win(win_mem + warp * WinSlab<LPR>::kBytes, grp);
-
     if (threadIdx.x == 0) {            // the map comes from the device-resident level table: no host read, capture-safe
         int run = 0, href = 0, wref = 0;
         bool tiled = (Lq == S);
@@ -160,8 +142,12 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                           : (npairs + kRegionIterSlots - 1) / kRegionIterSlots;
     }
     __syncthreads();
-    pdl_wait_primary();      // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
 
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane % LPR, grp = lane / LPR;
+    const int LP = L * P;
+    const unsigned row_elems = (unsigned)(M * D);
+    TapSlab<LPR> slab(slab_mem + warp * TapSlab<LPR>::kBytes, grp);
     for (unsigned tile = blockIdx.x; tile < rm.ntiles; tile += gridDim.x) {
         // ---- tile geometry: thread l resolves level l, thread 0 then lays the levels out ----
         if (rm.region) {
@@ -192,32 +178,18 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                 }
                 tl.qpre[L] = nq; tl.wbase[L] = nw;
                 tl.nq = nq; tl.nwin = nw;
-                int sf = nw;               // stage whole levels from the last one down while they fit
-                for (int k = L - 1; k >= 0 && nw - tl.wbase[k] <= kRegionStageRows; --k) sf = tl.wbase[k];
-                tl.sfirst = sf;
             }
         } else if (threadIdx.x == 0) {
             tl.base_pair = tile * kRegionIterSlots;
             tl.nq = (int)min((unsigned)kRegionIterSlots, npairs - tl.base_pair);
-            tl.nwin = tl.sfirst = 0;
+            tl.nwin = 0;
         }
         __syncthreads();
-        // ---- staging: window rows [sfirst, nwin), one 16-byte cp.async per lane and row slice ----
-        const int sfirst = tl.sfirst;
-        for (int i = threadIdx.x; i < (tl.nwin - sfirst) * LPR; i += kTiledThreads) {
-            const int r = sfirst + i / LPR;
-            int l = L - 1;
-            while (r < tl.wbase[l]) --l;
-            const int k = r - tl.wbase[l], y = tl.wy0[l] + k / tl.ww[l], x = tl.wx0[l] + k % tl.ww[l];
-            const int row = rm.start[l] + y * rm.W[l] + x;
-            cp_async16(vstage + i, value + (((size_t)tl.b * S + row) * M + tl.m) * D + (size_t)(i % LPR) * VEC);
-        }
         for (int i = threadIdx.x; i < tl.nwin; i += kTiledThreads) cnt[i] = 0;
-        cp_async_wait_all();
         __syncthreads();
-        MSDA_REGION_CLOCK(0);
+        MSDA_REGION_CLOCK(1);
 
-        // ---- phase A: gathers, grad_loc / grad_attn; in-window corners become entries, the others red ----
+        // ---- phase A: in-window corners become entries, the others red ----
 #pragma unroll 1
         for (int it = 0; it * kRegionIterSlots < tl.nq; ++it) {
             const int slot = it * kRegionIterSlots + warp * GPW + grp;
@@ -242,27 +214,28 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
             if (active) RowVec<float, VEC>::load(grad_out + (size_t)pair * D + (size_t)sub * VEC, g);
             if (stash) gstash[slot * LPR + sub] = make_float4(g[0], g[1], g[2], g[3]);
 
-            // ---- stage 1: this lane resolves taps sub, sub + LPR (dead taps: zero weight, row 0, no window) ----
-            float4 tw[NSL];
-            int2 tr[NSL], twin[NSL];
-            float tlh[NSL], tlw[NSL], ta[NSL];
-            unsigned tmeta[NSL];
+            // ---- this lane resolves taps sub, sub + LPR and files their in-window corners; the rest go to the slab ----
+            float4 tw[NSL];              // weights of the corners that red directly (the others 0)
+            int2 tr[NSL];
 #pragma unroll
             for (int k = 0; k < NSL; ++k) {
                 const int s = sub + k * LPR;
                 tw[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-                tr[k] = twin[k] = make_int2(0, 0);
-                tlh[k] = tlw[k] = ta[k] = 0.f; tmeta[k] = 0;
+                tr[k] = make_int2(0, 0);
+                unsigned filed = 0;
+                ushort4 rows4 = make_ushort4(kNoRow, kNoRow, kNoRow, kNoRow);
+                float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (s < LP && active) {
                     const size_t t = (size_t)pair * LP + s;
                     const float2 xy = __ldg(reinterpret_cast<const float2 *>(loc) + t);
                     const float a = __ldg(attn + t);
                     const int l = s / P;
                     const TapGeom gm = tap_geometry(xy.x, xy.y, rm.H[l], rm.W[l], rm.start[l]);
-                    tw[k] = masked_weights(gm, a);
+                    w4 = masked_weights(gm, a);
                     tr[k] = make_int2(gm.r0, gm.r1 | (gm.dw << 31));
-                    tlh[k] = gm.lh; tlw[k] = gm.lw; ta[k] = a; tmeta[k] = gm.mask | ((unsigned)l << 4);
-                    if (rm.region) {
+                    const unsigned nz = (unsigned)(w4.x != 0.f) | ((unsigned)(w4.y != 0.f) << 1) |
+                                        ((unsigned)(w4.z != 0.f) << 2) | ((unsigned)(w4.w != 0.f) << 3);
+                    if (stash) {
                         const int W = rm.W[l], o0 = gm.r0 - rm.start[l], o1 = gm.r1 - rm.start[l];
                         const int y0 = o0 / W, x0 = o0 - y0 * W, y1 = o1 / W;
                         const int wwl = tl.ww[l], whl = tl.wh[l];
@@ -270,76 +243,53 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                         const unsigned iy0 = (unsigned)ry0 < (unsigned)whl, iy1 = (unsigned)ry1 < (unsigned)whl;
                         const unsigned ix0 = (unsigned)rx0 < (unsigned)wwl, ix1 = (unsigned)rx1 < (unsigned)wwl;
                         const unsigned inwin = (iy0 & ix0) | ((iy0 & ix1) << 1) | ((iy1 & ix0) << 2) | ((iy1 & ix1) << 3);
-                        const int staged = tl.wbase[l] >= tl.sfirst;
-                        twin[k] = make_int2(tl.wbase[l] + ry0 * wwl + rx0,
-                                            (((y1 - y0) * wwl) << 6) | (staged << 5) | (gm.dw << 4) | (int)inwin);
+                        filed = inwin & nz;
+                        const int w00 = tl.wbase[l] + ry0 * wwl + rx0, dhw = (y1 - y0) * wwl;
+                        const int wr[4] = {w00, w00 + gm.dw, w00 + dhw, w00 + dhw + gm.dw};
+#pragma unroll
+                        for (int c = 0; c < 4; ++c)
+                            if ((filed >> c) & 1u) atomicAdd(&cnt[wr[c]], 1);      // phase B's row count; result unused
+                        rows4 = make_ushort4((filed & 1u) ? (unsigned short)wr[0] : kNoRow,
+                                             (filed & 2u) ? (unsigned short)wr[1] : kNoRow,
+                                             (filed & 4u) ? (unsigned short)wr[2] : kNoRow,
+                                             (filed & 8u) ? (unsigned short)wr[3] : kNoRow);
                     }
+                    tw[k] = make_float4((filed & 1u) ? 0.f : w4.x, (filed & 2u) ? 0.f : w4.y,
+                                        (filed & 4u) ? 0.f : w4.z, (filed & 8u) ? 0.f : w4.w);
+                }
+                if (stash) {
+                    const int e = (slot * LP_MAX + s) << 2;
+                    *reinterpret_cast<ushort4 *>(e_row + e) = rows4;
+                    *reinterpret_cast<float4 *>(e_coef + e) = w4;
                 }
             }
 
+            // ---- direct reds: the group walks the taps of its pair that have a corner to red ----
             const size_t slab_off = ((size_t)b * S * M + m) * D + (size_t)sub * VEC;
-            const float *base = value + slab_off;
             float *gbase = grad_value + slab_off;
-
-            // ---- stage 2 ----
 #pragma unroll
             for (int k = 0; k < NSL; ++k) {
                 __syncwarp();
                 slab.put(sub, tw[k], tr[k]);
-                win.put(sub, twin[k]);
                 __syncwarp();
-                float part[LPR][4];
-#pragma unroll
-                for (int j = 0; j < LPR; ++j) {
+                const bool any = tw[k].x != 0.f || tw[k].y != 0.f || tw[k].z != 0.f || tw[k].w != 0.f;
+                unsigned todo = (__ballot_sync(kFullMask, any) >> (grp * LPR)) & ((1u << LPR) - 1u);
+                while (todo) {
+                    const int j = __ffs(todo) - 1;
+                    todo &= todo - 1u;
                     const float4 w4 = slab.weights(j);
                     const int2 rr = slab.rows(j);
-                    const int2 wi = win.get(j);
                     const float w[4] = {w4.x, w4.y, w4.z, w4.w};
-                    const unsigned nz = (unsigned)(w4.x != 0.f) | ((unsigned)(w4.y != 0.f) << 1) |
-                                        ((unsigned)(w4.z != 0.f) << 2) | ((unsigned)(w4.w != 0.f) << 3);
-                    // corners that become entries / that are read from the staged rows (both group-uniform)
-                    const unsigned ok = stash ? (unsigned)wi.y & nz & 15u : 0u;
-                    const unsigned sm = (wi.y & 32) ? (unsigned)wi.y & 15u : 0u;
-                    const int dw = (wi.y >> 4) & 1, dhw = wi.y >> 6;
-                    if (stash && sub < 4) {                                   // lane c files corner c of tap j
-                        const int wrow = wi.x + ((sub & 1) ? dw : 0) + ((sub & 2) ? dhw : 0);
-                        const int e = ((slot * LP_MAX + k * LPR + j) << 2) + sub;
-                        const bool filed = (ok >> sub) & 1u;
-                        e_row[e] = filed ? (unsigned short)wrow : kNoRow;
-                        e_coef[e] = sub == 0 ? w4.x : sub == 1 ? w4.y : sub == 2 ? w4.z : w4.w;
-                        if (filed) atomicAdd(&cnt[wrow], 1);                  // phase B's row count; result unused
-                    }
                     const unsigned dwo = (rr.y < 0) ? row_elems : 0u;
                     unsigned long long off[4];
                     off[0] = (unsigned long long)(unsigned)rr.x * row_elems;
                     off[1] = off[0] + dwo;
                     off[2] = (unsigned long long)(unsigned)(rr.y & 0x7fffffff) * row_elems;
                     off[3] = off[2] + dwo;
-                    const float4 *srow = vstage + (wi.x - sfirst) * LPR + sub;   // corner 00's staged row (if staged)
 #pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        float v[VEC];
-                        if ((sm >> c) & 1u) {
-                            const float4 t = srow[(((c & 1) ? dw : 0) + ((c & 2) ? dhw : 0)) * LPR];
-                            v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
-                        } else {
-                            RowVec<float, VEC>::load(base + off[c], v);
-                        }
-                        float dsum = 0.f;
-#pragma unroll
-                        for (int e = 0; e < VEC; ++e) dsum = fmaf(g[e], v[e], dsum);
-                        part[j][c] = dsum;
-                        if (w[c] != 0.f && !((ok >> c) & 1u) && MSDA_REGION_KEEP_RED(1))
+                    for (int c = 0; c < 4; ++c)
+                        if (w[c] != 0.f && MSDA_REGION_KEEP_RED(1))
                             red_add_v4(gbase + off[c], w[c] * g[0], w[c] * g[1], w[c] * g[2], w[c] * g[3]);
-                    }
-                }
-                float dot[4];
-                group_reduce_scatter<LPR>(part, sub, dot);
-                const int s = sub + k * LPR;
-                if (s < LP && active) {
-                    const int l = (int)(tmeta[k] >> 4);
-                    finish_tap(dot, tmeta[k], tlh[k], tlw[k], ta[k], rm.H[l], rm.W[l], (size_t)pair * LP + s, grad_loc,
-                               grad_attn);
                 }
             }
         }
@@ -347,7 +297,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
         const int nwin = tl.nwin;
         if (nwin > 0) {
             __syncthreads();
-            MSDA_REGION_CLOCK(1);
+            MSDA_REGION_CLOCK(2);
             const int n = min(tl.nq, kRegionSlots) * LP_MAX * 4;
             // ---- phase B: counting sort of the entries by window row (phase A counted them) ----
             {   // exclusive scan of cnt[0, nwin): 4 rows per thread
@@ -380,7 +330,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
                 }
             }
             __syncthreads();          // bucket r is now [r ? cnt[r - 1] : 0, cnt[r]) of s_coef / s_slot
-            MSDA_REGION_CLOCK(2);
+            MSDA_REGION_CLOCK(3);
 
             // ---- phase C: one group per touched row, one red per lane ----
             const int b = tl.b, m = tl.m;
@@ -404,8 +354,38 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
             }
         }
         __syncthreads();              // the next tile rewrites tl, the entry list, the stash and the counts
-        MSDA_REGION_CLOCK(nwin > 0 ? 3 : 1);
+        MSDA_REGION_CLOCK(nwin > 0 ? 4 : 2);
     }
+}
+
+// tma: the tap pass stages (x, y, a) with TMA (use_tma_staging on the host: L*P % 4 == 0).
+template <int R, int HALO>
+__global__ void __launch_bounds__(kTiledThreads, kRegionMinCtas)
+msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ value,
+                const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
+                const float *__restrict__ loc, const float *__restrict__ attn,
+                int N, int S, int M, int L, int Lq, int P, unsigned npairs, int tma,
+                float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn)
+{
+    __shared__ WorkMap wm;
+    __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<8>::kBytes];
+    __shared__ __align__(8) unsigned long long stage_bar[kTiledWarps * 2];
+    extern __shared__ __align__(128) unsigned char region_dyn[];       // the stage buffers overlay the entry arrays
+
+    MSDA_REGION_CLOCK_INIT;
+    // ---- tap pass: grad_loc / grad_attn (writes nothing the zero-fill writes, so it overlaps the fill) ----
+    if (tma)
+        bwd_tiled_body<float, 4, 32, 16, true, false, false, true, false>(
+            wm, slab_mem, region_dyn, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
+            nullptr, grad_loc, grad_attn, nullptr, 0);
+    else
+        bwd_tiled_body<float, 4, 32, 16, false, false, false, true, false>(
+            wm, slab_mem, region_dyn, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
+            nullptr, grad_loc, grad_attn, nullptr, 0);
+    __syncthreads();         // the stage buffers are free again
+    MSDA_REGION_CLOCK(0);
+    pdl_wait_primary();      // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
+    region_grad_value_pass<R, HALO>(grad_out, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, grad_value);
 }
 
 }  // namespace msda

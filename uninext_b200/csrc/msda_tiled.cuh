@@ -404,10 +404,17 @@ __device__ __forceinline__ void finish_tap(const float (&dot)[4], unsigned mk, f
 // bytes through the SM's crossbar port, which is what bounds this kernel -- while the coarse levels (hundreds to
 // thousands of contributions per row) keep the fp32 accumulator.  The fine flag travels in bit 31 of the record's row
 // index (rows are < 2^30).
-// NORED: grad_loc / grad_attn only, grad_value untouched (the deterministic backward sums grad_value itself, msda_det.cuh).
-template <typename T, int VEC, int D, int LP_MAX, int MIN_CTAS, bool TMA, bool SPLIT, bool MIXED = false, bool NORED = false>
-__global__ void __launch_bounds__(kTiledThreads, MIN_CTAS)
-msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
+// NORED: grad_loc / grad_attn only, grad_value untouched (the deterministic backward sums grad_value itself, msda_det.cuh;
+// the region backward's tap pass, msda_region.cuh).
+//
+// The body is a device function so that msda_bwd_region runs the same code, in the same FMA order, as its tap pass.  The
+// caller owns the shared memory: the work map, kTiledWarps tap slabs, kTiledWarps * TapStage::kBytes of 16-byte aligned
+// stage buffers (TMA) and 2 * kTiledWarps mbarriers.  WAIT_PRIMARY: wait for the PDL primary (grad_value's zero-fill)
+// before the first tile.
+template <typename T, int VEC, int D, int LP_MAX, bool TMA, bool SPLIT, bool MIXED, bool NORED, bool WAIT_PRIMARY>
+__device__ __forceinline__ void
+bwd_tiled_body(WorkMap &wm, unsigned char *slab_mem, unsigned char *stage_mem, unsigned long long *stage_bar,
+               const T *__restrict__ grad_out, const T *__restrict__ value,
                const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
                const float *__restrict__ loc, const float *__restrict__ attn,
                int N, int S, int M, int L, int Lq, int P, unsigned npairs, int allow_patches,
@@ -425,8 +432,6 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
     static_assert(D % VEC == 0 && (LPR & (LPR - 1)) == 0 && LPR <= 32 && LP_MAX % LPR == 0, "bad tiling");
     static_assert(!SPLIT || (LP_MAX % GPW == 0 && LP_MAX / GPW <= LPR && !TMA), "SPLIT: one record round, LDG taps");
 
-    __shared__ WorkMap wm;
-    __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<LPR>::kBytes];
     build_work_map(wm, shapes, lsi, L, N, S, Lq, M, npairs, SPLIT ? 0 : allow_patches, kTiledWarps * PPW);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -437,8 +442,6 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
 
     // per-warp TMA double buffer for (x, y, a) -- linear order only (the host passes TMA=true only then)
     using Stage = TapStage<GPW, LP_MAX, TMA>;
-    __shared__ __align__(128) unsigned char stage_mem[kTiledWarps * Stage::kBytes];
-    __shared__ __align__(8) unsigned long long stage_bar[kTiledWarps * 2];
     unsigned char *my_stage = stage_mem + warp * Stage::kBytes;
     unsigned long long *my_bar = stage_bar + warp * 2;
     unsigned tma_iter = 0;
@@ -461,7 +464,8 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
         }
         __syncwarp();
     }
-    pdl_wait_primary();      // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
+    if constexpr (WAIT_PRIMARY)
+        pdl_wait_primary();  // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
 
     for (unsigned tile = blockIdx.x; tile < wm.ntiles; tile += gridDim.x) {
         const TileCtx tc = decode_tile(wm, tile, L, M);
@@ -571,6 +575,24 @@ msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
             }
         }
     }
+}
+
+template <typename T, int VEC, int D, int LP_MAX, int MIN_CTAS, bool TMA, bool SPLIT, bool MIXED = false, bool NORED = false>
+__global__ void __launch_bounds__(kTiledThreads, MIN_CTAS)
+msda_bwd_tiled(const T *__restrict__ grad_out, const T *__restrict__ value,
+               const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
+               const float *__restrict__ loc, const float *__restrict__ attn,
+               int N, int S, int M, int L, int Lq, int P, unsigned npairs, int allow_patches,
+               float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn,
+               __nv_bfloat16 *__restrict__ grad_value_bf16, int fine_min_rows)
+{
+    __shared__ WorkMap wm;
+    __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<D / VEC>::kBytes];
+    __shared__ __align__(128) unsigned char stage_mem[kTiledWarps * TapStage<32 / (D / VEC), LP_MAX, TMA>::kBytes];
+    __shared__ __align__(8) unsigned long long stage_bar[kTiledWarps * 2];
+    bwd_tiled_body<T, VEC, D, LP_MAX, TMA, SPLIT, MIXED, NORED, true>(
+        wm, slab_mem, stage_mem, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs,
+        allow_patches, grad_value, grad_loc, grad_attn, grad_value_bf16, fine_min_rows);
 }
 
 }  // namespace msda
