@@ -184,13 +184,18 @@ int msda_backward_det_bf16(const uint16_t *grad_out, const uint16_t *value,
  *   proj [R, M*L*P*3]: columns [0, M*L*P*2) = sampling offsets ordered (m,l,p,xy) (ms_deform_attn.py:99),
  *                      columns [M*L*P*2, M*L*P*3) = attention logits ordered (m, l*p) (ms_deform_attn.py:100);
  *   ref  [R, L, refdim] reference points (refdim 2) or boxes (refdim 4) (ms_deform_attn.py:103-109); R = N*Lq;
- *   loc  [R, M, L, P, 2], attn [R, M, L, P] outputs.  L*P <= 32.
+ *   loc  [R, M, L, P, 2], attn [R, M, L, P] outputs.  L*P <= 32.  loc is written as float2: 8-byte aligned.
  * msda_prologue_backward_f32: gradient of the raw projection from grad_loc / grad_attn (reference points are
- *   treated as constants).
+ *   treated as constants).  grad_loc is read as float2: 8-byte aligned.
  * msda_colsum_f32: out[c] = sum_r x[r,c] (bias gradients); cols % 4 == 0; `out` is zero-filled by the callee.
+ *   x and out 16-byte aligned (float4 loads, 16-byte reductions).
  * msda_add_layernorm_forward_f32 / msda_layernorm_backward_f32: y = LayerNorm(a + b) over the last dimension
  *   (deformable_transformer.py:354-356,359); cols in {128, 256, 384, 512}; b and z may be NULL (z = a + b is needed by
- *   the backward when b != NULL); dgamma / dbeta are zero-filled by the callee. */
+ *   the backward when b != NULL; without b a non-NULL z receives a copy of a); dgamma / dbeta are zero-filled by the
+ *   callee.  Every row is accessed as float4: a, b, gamma, beta, z, y (forward) and dy, z, gamma, dz, dgamma, dbeta
+ *   (backward) must be 16-byte aligned where non-NULL; mean / rstd need natural alignment only.
+ * For all of these an operand that misses its alignment -- e.g. a contiguous view with a storage offset -- is
+ * MSDA_E_BADARG, returned before anything is enqueued; callers copy such an operand or use another implementation. */
 int msda_prologue_forward_f32(const float *proj, const float *ref, const int64_t *spatial_shapes,
                               int64_t R, int M, int L, int P, int refdim, float *loc, float *attn, void *stream);
 int msda_prologue_backward_f32(const float *grad_loc, const float *grad_attn, const float *attn, const float *ref,
@@ -198,7 +203,8 @@ int msda_prologue_backward_f32(const float *grad_loc, const float *grad_attn, co
                                float *grad_proj, void *stream);
 int msda_colsum_f32(const float *x, int64_t rows, int cols, float *out, void *stream);
 /* ReLU backward fused with the bias gradient of the Linear before it (FFN linear1): g2 = g where y > 0 else 0;
- * colsum[c] = sum_r g2[r, c] (zero-filled by the callee).  cols % 4 == 0. */
+ * colsum[c] = sum_r g2[r, c] (zero-filled by the callee).  cols % 4 == 0; g, y, g2 and colsum 16-byte aligned
+ * (float4 accesses), otherwise MSDA_E_BADARG. */
 int msda_relu_backward_colsum_f32(const float *g, const float *y, int64_t rows, int cols, float *g2, float *colsum, void *stream);
 int msda_add_layernorm_forward_f32(const float *a, const float *b, const float *gamma, const float *beta,
                                    int64_t rows, int cols, float eps, float *z, float *y, float *mean, float *rstd,
@@ -233,7 +239,8 @@ int msda_sine_pos_embed_backward_f32(const float *pos, const float *grad_out, in
  *     refs [I, 2] reference points in input-image pixels; inst_start [N + 1] int32 (device): instances of image b are
  *     [inst_start[b], inst_start[b+1]); max_inst = largest per-image count (host value, sizes the grid);
  *     stride = mask_feat_stride; rel_coord = 1 prepends (ref - pixel location) as two input channels, 0 feeds zeros;
- *     logits [I, H, W].
+ *     logits [I, H, W].  Any element-aligned feats / logits are accepted: 16-byte accesses are used only when
+ *     H*W % 4 == 0 and both pointers are 16-byte aligned, scalar ones otherwise (same results).
  * msda_condinst_backward_f32: grad_feats [N, 8, H, W], grad_params [I, 169] and grad_refs [I, 2] (all zero-filled by the
  *   callee, then accumulated with fp32 reductions: summation order, hence the last bits, vary from run to run).
  * msda_aligned_bilinear_forward/backward_f32: `aligned_bilinear` (ddetrs.py:921-942) on [planes, h, w] -> [planes, f*h, f*w]. */

@@ -28,6 +28,7 @@ std::atomic<uint64_t> g_launches{0};
 struct Dims { int N, S, M, D, L, Lq, P; };
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+inline bool aligned8(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 
 int check_dims(const Dims &d) {
     if (d.N <= 0 || d.S <= 0 || d.M <= 0 || d.D <= 0 || d.L <= 0 || d.Lq <= 0 || d.P <= 0) return MSDA_E_BADARG;
@@ -894,7 +895,7 @@ extern "C" {
 int msda_prologue_forward_f32(const float *proj, const float *ref, const int64_t *spatial_shapes, int64_t R, int M, int L,
                               int P, int refdim, float *loc, float *attn, void *stream) {
     if (!proj || !ref || !spatial_shapes || !loc || !attn || R <= 0 || M <= 0 || L <= 0 || P <= 0 || L * P > 32 ||
-        (refdim != 2 && refdim != 4) || (long long)R * M * 32 >= (1ll << 40))
+        (refdim != 2 && refdim != 4) || (long long)R * M * 32 >= (1ll << 40) || !aligned8(loc))      // float2 stores
         return MSDA_E_BADARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long np = (long long)R * M;
@@ -910,7 +911,7 @@ int msda_prologue_backward_f32(const float *grad_loc, const float *grad_attn, co
                                const int64_t *spatial_shapes, int64_t R, int M, int L, int P, int refdim,
                                float *grad_proj, void *stream) {
     if (!grad_loc || !grad_attn || !attn || !ref || !spatial_shapes || !grad_proj || R <= 0 || M <= 0 || L <= 0 || P <= 0 ||
-        L * P > 32 || (refdim != 2 && refdim != 4))
+        L * P > 32 || (refdim != 2 && refdim != 4) || !aligned8(grad_loc))                             // float2 loads
         return MSDA_E_BADARG;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long np = (long long)R * M;
@@ -956,6 +957,8 @@ int msda_add_layernorm_forward_f32(const float *a, const float *b, const float *
                                    int cols, float eps, float *z, float *y, float *mean, float *rstd, void *stream) {
     if (!a || !gamma || !beta || !y || !mean || !rstd || rows <= 0 || (b != nullptr && z == nullptr)) return MSDA_E_BADARG;
     if (cols != 128 && cols != 256 && cols != 384 && cols != 512) return MSDA_E_BADARG;
+    if (!aligned16(a) || !aligned16(gamma) || !aligned16(beta) || !aligned16(y) || (b && !aligned16(b)) || (z && !aligned16(z)))
+        return MSDA_E_BADARG;                                                                        // float4 accesses
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const unsigned grid = (unsigned)((rows + 7) / 8);
     switch (cols / 128) {
@@ -972,6 +975,8 @@ int msda_layernorm_backward_f32(const float *dy, const float *z, const float *ga
                                 int64_t rows, int cols, float *dz, float *dgamma, float *dbeta, void *stream) {
     if (!dy || !z || !gamma || !mean || !rstd || !dz || !dgamma || !dbeta || rows <= 0) return MSDA_E_BADARG;
     if (cols != 128 && cols != 256 && cols != 384 && cols != 512) return MSDA_E_BADARG;
+    if (!aligned16(dy) || !aligned16(z) || !aligned16(gamma) || !aligned16(dz) || !aligned16(dgamma) || !aligned16(dbeta))
+        return MSDA_E_BADARG;                                                                        // float4 accesses, 16-byte reds
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaError_t err = cudaMemsetAsync(dgamma, 0, sizeof(float) * (size_t)cols, st);
     if (err == cudaSuccess) err = cudaMemsetAsync(dbeta, 0, sizeof(float) * (size_t)cols, st);
@@ -1003,8 +1008,11 @@ int msda_condinst_forward_f32(const float *feats, const float *params, const flo
     if (I == 0 || max_inst == 0) return 0;
     const int HW = H * W, tile = msda::kCiFwdThreads * msda::kCiFwdPpt;
     const dim3 grid((unsigned)((HW + tile - 1) / tile), (unsigned)((max_inst + msda::kCiChunk - 1) / msda::kCiChunk), (unsigned)N);
+    // 16-byte accesses need every row of feats / logits 16-byte aligned: HW % 4 == 0 and aligned base pointers (a view with a
+    // storage offset is not); anything else takes the scalar path
+    const int vec = HW % 4 == 0 && aligned16(feats) && aligned16(logits);
     msda::condinst_fwd<<<grid, msda::kCiFwdThreads, 0, static_cast<cudaStream_t>(stream)>>>(feats, params, refs, inst_start, HW,
-                                                                                          W, stride, rel_coord, logits);
+                                                                                          W, stride, rel_coord, vec, logits);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return (int)cudaGetLastError();
 }

@@ -145,10 +145,12 @@ __device__ __forceinline__ float ci_loc(int px, int W, int stride, bool want_y) 
 // ---- forward: a pair = two neighbouring pixels of one instance; a thread owns kCiFwdGroups groups of 4 consecutive pixels,
 // group g of thread t at pixel (tile * groups + g) * 4 * blockDim + 4 * t, so every 16-byte access of a warp is contiguous.
 // grid: (pixel tiles, instance chunks, images).  feats [N, 8, H*W]; params [I, 169]; refs [I, 2] (pixels of the input image);
-// inst_start [N + 1] (instances of image b are [inst_start[b], inst_start[b + 1])); logits [I, H*W].
+// inst_start [N + 1] (instances of image b are [inst_start[b], inst_start[b + 1])); logits [I, H*W].  vec (host-decided:
+// HW % 4 == 0 and feats / logits 16-byte aligned): a live group has 4 pixels and every row is 16-byte aligned, so each group
+// is one float4 load per channel and one float4 store per instance; otherwise scalar accesses with per-pixel bounds.
 __global__ void __launch_bounds__(kCiFwdThreads)
 condinst_fwd(const float *__restrict__ feats, const float *__restrict__ params, const float *__restrict__ refs,
-             const int *__restrict__ inst_start, int HW, int W, int stride, int rel_coord, float *__restrict__ logits)
+             const int *__restrict__ inst_start, int HW, int W, int stride, int rel_coord, int vec, float *__restrict__ logits)
 {
     constexpr int G = kCiFwdGroups, NP = 2 * G;
     __shared__ __align__(16) float sp[kCiChunk][kCiRow];
@@ -164,7 +166,6 @@ condinst_fwd(const float *__restrict__ feats, const float *__restrict__ params, 
 #pragma unroll
     for (int g = 0; g < G; ++g) gpx[g] = ((blockIdx.x * G + g) * kCiFwdThreads + threadIdx.x) * 4;
     if (gpx[0] >= HW) return;
-    const bool vec = (HW & 3) == 0;            // then a live group has 4 pixels and every row of feats / logits is 16-byte aligned
     f2 x[NP][kCiIn], lx[NP], ly[NP];
 #pragma unroll
     for (int g = 0; g < G; ++g) {

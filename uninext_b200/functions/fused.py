@@ -33,6 +33,13 @@ def _f32c(t):
     return t.contiguous() if t.dtype == torch.float32 else t.float().contiguous()
 
 
+def _aligned(t, align=16):
+    """``t`` itself, or a fresh copy when its data pointer is not ``align``-byte aligned.  A contiguous view with a storage
+    offset (e.g. the gradient autograd hands on from a ``torch.cat`` of flattened tensors) stays a view through
+    ``contiguous()`` / ``reshape``; the vector kernels cannot read it, the caching allocator's fresh blocks they can."""
+    return t if t.data_ptr() % align == 0 else t.clone()
+
+
 def colsum(x2d: torch.Tensor) -> torch.Tensor:
     """sum over rows of a contiguous fp32 [rows, cols] CUDA tensor (cols % 4 == 0)."""
     rows, cols = x2d.shape
@@ -153,10 +160,13 @@ class _LinearColsum(Function):
         x2, weight, y, mask = ctx.saved_tensors
         g2 = g.reshape(-1, g.shape[-1])
         gb = None
-        if ctx.relu and g2.is_cuda and g2.dtype == torch.float32 and g2.shape[1] % 4 == 0 and ctx.needs_input_grad[2] \
-                and not deterministic_requested():
-            # ReLU backward and the bias gradient in ONE pass over (g, y)  (masked rows have y == 0: zeroed by the same test)
+        fused_relu = ctx.relu and g2.is_cuda and g2.dtype == torch.float32 and g2.shape[1] % 4 == 0 \
+            and ctx.needs_input_grad[2] and not deterministic_requested()
+        if fused_relu:
             g2 = g2.contiguous()
+            fused_relu = g2.data_ptr() % 16 == 0 and y.data_ptr() % 16 == 0        # float4 kernel; else as colsum() does
+        if fused_relu:
+            # ReLU backward and the bias gradient in ONE pass over (g, y)  (masked rows have y == 0: zeroed by the same test)
             out = torch.empty_like(g2)
             gb = torch.empty(g2.shape[1], dtype=torch.float32, device=g2.device)
             with torch.cuda.device(g2.device):
@@ -257,7 +267,7 @@ class _SamplingPrologue(Function):
         m, l, p, rd, n_off, qshape = ctx.dims
         rows = q2.shape[0]
         g_proj = torch.empty((rows, weight.shape[0]), dtype=torch.float32, device=q2.device)
-        g_loc, g_attn = _f32c(g_loc), _f32c(g_attn)
+        g_loc, g_attn = _aligned(_f32c(g_loc), 8), _f32c(g_attn)             # grad_loc is read as float2
         with torch.cuda.device(q2.device):
             _cabi.check(lib.msda_prologue_backward_f32(g_loc.data_ptr(), g_attn.data_ptr(), attn.data_ptr(), ref_c.data_ptr(),
                                                        shapes.data_ptr(), rows, m, l, p, rd, g_proj.data_ptr(), _stream()),
@@ -307,7 +317,7 @@ class _AddLayerNorm(Function):
         lib = _cabi.load()
         z, gamma, mean, rstd = ctx.saved_tensors
         rows, cols = z.shape
-        gy2 = _f32c(gy.reshape(rows, cols))
+        gy2 = _aligned(_f32c(gy.reshape(rows, cols)))
         dz = torch.empty_like(z)
         dgamma = torch.empty_like(gamma)
         dbeta = torch.empty_like(gamma)
