@@ -1,4 +1,4 @@
-"""GPU tests of the fused image-text attention in bf16 mode (msda_vlfuse_bf16.cuh): taken for bf16 q, k, vv and vl.
+"""GPU tests of the fused image-text attention in bf16 mode (msda_vlfuse_tc.cuh): taken for bf16 q, k, vv and vl.
 
 Accuracy is judged against bf16 products: the yardstick restates the kernels' formulas in torch with every product
 operand rounded to bf16, fp32 accumulation and the outputs rounded to bf16 (``_bf16_model``, the bf16 counterpart of

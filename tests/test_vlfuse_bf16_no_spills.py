@@ -1,4 +1,4 @@
-"""CPU test: the bf16 tensor-core kernels of the fused image-text attention (msda_vlfuse_bf16.cuh) are in the compiler's
+"""CPU test: the bf16 tensor-core kernels of the fused image-text attention (msda_vlfuse_tc.cuh) are in the compiler's
 report in uninext_b200/lib/build.log, for both head sizes, without register spills.  Skipped when the library has not
 been built."""
 import os

@@ -19,7 +19,6 @@
 #include "msda_tiled.cuh"
 #include "msda_vlfuse.cuh"
 #include "msda_vlfuse_tc.cuh"
-#include "msda_vlfuse_bf16.cuh"
 
 namespace {
 
@@ -1451,33 +1450,33 @@ cudaError_t vlf_backward_launch(const vlf::ParamsT<T> &p, const VlfLayout &l, vo
     return cudaGetLastError();
 }
 
-// The product kernels of each mode: F32 (msda_vlfuse.cuh), TF32 (msda_vlfuse_tc.cuh), BF16 (msda_vlfuse_bf16.cuh).
+// The product kernels of each mode: F32 (msda_vlfuse.cuh), TF32 and BF16 (msda_vlfuse_tc.cuh).
 enum VlfMode { kVlfF32, kVlfTF32, kVlfBF16 };
 
 template <int D>
 cudaError_t vlf_forward_mode(const vlf::Params &p, const VlfLayout &l, VlfMode mode, cudaStream_t st) {
     if (mode == kVlfTF32)
-        return vlf_forward_launch<D>(p, l, vlf::vlf_tc_fwd_rows<D>, vlf::kTcFwdRowsSmem, vlf::vlf_tc_fwd_cols<D>,
-                                     vlf::kTcFwdColsSmem, st);
+        return vlf_forward_launch<D>(p, l, vlf::vlf_tc_fwd_rows<D>, vlf::FwdRowsSmem<vlf::Tf32>::kBytes,
+                                     vlf::vlf_tc_fwd_cols<D>, vlf::FwdColsSmem<vlf::Tf32>::kBytes, st);
     return vlf_forward_launch<D>(p, l, vlf::vlf_fwd_rows<D>, vlf::kFwdRowsSmem, vlf::vlf_fwd_cols<D>, vlf::kFwdColsSmem, st);
 }
 template <int D>
 cudaError_t vlf_forward_mode(const vlf::ParamsH &p, const VlfLayout &l, VlfMode, cudaStream_t st) {
-    return vlf_forward_launch<D>(p, l, vlf::vlf_bf16_fwd_rows<D>, vlf::kH_FwdRowsSmem, vlf::vlf_bf16_fwd_cols<D>,
-                                 vlf::kH_FwdColsSmem, st);
+    return vlf_forward_launch<D>(p, l, vlf::vlf_bf16_fwd_rows<D>, vlf::FwdRowsSmem<vlf::Bf16>::kBytes,
+                                 vlf::vlf_bf16_fwd_cols<D>, vlf::FwdColsSmem<vlf::Bf16>::kBytes, st);
 }
 template <int D>
 cudaError_t vlf_backward_mode(const vlf::Params &p, const VlfLayout &l, VlfMode mode, cudaStream_t st) {
     if (mode == kVlfTF32)
-        return vlf_backward_launch<D>(p, l, vlf::vlf_tc_bwd_rows<D>, vlf::kTcBwdRowsSmem, vlf::vlf_tc_bwd_cols<D>,
-                                      vlf::kTcBwdColsSmem, st);
+        return vlf_backward_launch<D>(p, l, vlf::vlf_tc_bwd_rows<D>, vlf::BwdRowsSmem<vlf::Tf32>::kBytes,
+                                      vlf::vlf_tc_bwd_cols<D>, vlf::BwdColsSmem<vlf::Tf32>::kBytes, st);
     return vlf_backward_launch<D>(p, l, vlf::vlf_bwd_rows<D>, vlf::kBwdRowsSmem, vlf::vlf_bwd_cols<D>, vlf::kBwdColsSmem,
                                   st);
 }
 template <int D>
 cudaError_t vlf_backward_mode(const vlf::ParamsH &p, const VlfLayout &l, VlfMode, cudaStream_t st) {
-    return vlf_backward_launch<D>(p, l, vlf::vlf_bf16_bwd_rows<D>, vlf::kH_BwdRowsSmem, vlf::vlf_bf16_bwd_cols<D>,
-                                  vlf::kH_BwdColsSmem, st);
+    return vlf_backward_launch<D>(p, l, vlf::vlf_bf16_bwd_rows<D>, vlf::BwdRowsSmem<vlf::Bf16>::kBytes,
+                                  vlf::vlf_bf16_bwd_cols<D>, vlf::BwdColsSmem<vlf::Bf16>::kBytes, st);
 }
 
 // The tensors' element type behind an ABI pointer type: float, or bf16 passed as uint16_t.

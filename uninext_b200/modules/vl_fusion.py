@@ -6,7 +6,7 @@ The attention core -- logits, both clamps, the masked vision softmax, the text s
 products -- runs in the fused CUDA kernels of msda_vlfuse.cuh (DESIGN.md section 3.11), which never store the
 [B*H, S, T] logits.  When torch allows TF32 matmuls (``allow_tf32``, ``set_float32_matmul_precision("high")`` or
 ``fp32_precision = "tf32"``) the kernels of msda_vlfuse_tc.cuh run its products on TF32 tensor cores instead.  On bf16
-inputs the kernels of msda_vlfuse_bf16.cuh run them on bf16 tensor cores; ``op_dtype=torch.bfloat16`` on the modules
+inputs the same kernels, in bf16 mode, run them on bf16 tensor cores; ``op_dtype=torch.bfloat16`` on the modules
 casts the core's inputs to bf16.  The six projections are cuBLAS GEMMs (``F.linear``).  ``vl_attention_torch`` restates
 the core with torch ops; it serves CPU tensors, ``stable_softmax_2d=True``, other dtypes and shapes outside the kernels'
 limits (head_dim 128 / 256, T <= 256).
