@@ -84,7 +84,8 @@ Knobs &knobs() { static Knobs k; return k; }
 int knob(int i) { return knobs().v[i].load(std::memory_order_relaxed); }
 
 // Set by msda_backward_* when the zero-fill just issued on the stream may be the PDL primary of the next launch; consumed
-// (and cleared) by launch_bwd, cleared by msda_backward_* on every other route.
+// (and cleared) by launch_after_fill, cleared by msda_backward_* on every other route.  Only kernels that wait for the
+// primary (pdl_wait_primary) before touching grad_value may be launched through launch_after_fill.
 thread_local bool t_pdl_next = false;
 
 // Zero-fill of grad_value before the backward kernels (MSDA_KNOB_ZERO_FILL).  *pdl is set when the fill went out as a
@@ -174,46 +175,6 @@ constexpr int kFwdMinCtas = 4, kBwdMinCtas = 2;     // r01d sweep: fwd flat for 
 template <typename T> struct FwdVec { static constexpr int v = 16 / sizeof(T); };      // 16-byte row slices
 template <typename T> struct BwdVec { static constexpr int v = 4; };                  // 4 channels per lane (see RowVec)
 
-template <typename T, int D, int LP_MAX, int VEC = FwdVec<T>::v>
-cudaError_t launch_fwd(const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc, const float *attn,
-                       const Dims &d, T *out, cudaStream_t st) {
-    constexpr int GPW = 32 / (D / VEC);
-    constexpr bool kCanStage = (LP_MAX <= 16);          // per-warp double buffer must fit static shared memory
-    constexpr bool kCanSplit = (LP_MAX % GPW == 0) && (LP_MAX / GPW <= D / VEC);
-    const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
-    const bool split = kCanSplit && use_split(npairs);
-    const bool tma = !split && kCanStage && use_tma_staging(d);
-    if constexpr (sizeof(T) == 2 && VEC == 8) {      // bf16: packed-bf16 corner blend for the large (non-split) launches
-        if (!split && knob(MSDA_KNOB_BF16_PACKED_FWD) == 1) {
-            static std::atomic<int> c_ptma[kMaxDevices], c_pldg[kMaxDevices];
-            auto k_tma = msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, kCanStage, false, true>;
-            auto k_ldg = msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false, true>;
-            const int pslots = tma ? resident_ctas_cached(k_tma, c_ptma) : resident_ctas_cached(k_ldg, c_pldg);
-            const unsigned ip = msda::kTiledWarps * GPW;
-            const unsigned tub = (npairs + ip - 1) / ip;
-            const int pgrid = (int)(tub < (unsigned)pslots ? tub : (unsigned)pslots);
-            (tma ? k_tma : k_ldg)<<<pgrid, msda::kTiledThreads, 0, st>>>(value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P,
-                                                                          npairs, allow_patches(), out);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            return cudaGetLastError();
-        }
-    }
-    auto kern = split ? msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, kCanSplit>
-                : tma ? msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, kCanStage, false>
-                      : msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false>;
-    static std::atomic<int> c_split[kMaxDevices], c_tma[kMaxDevices], c_ldg[kMaxDevices];
-    const int slots = split ? resident_ctas_cached(msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, kCanSplit>, c_split)
-                      : tma ? resident_ctas_cached(msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, kCanStage, false>, c_tma)
-                            : resident_ctas_cached(msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false>, c_ldg);
-    const unsigned iter_pairs = msda::kTiledWarps * (split ? 1 : GPW);
-    const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;        // linear order (patch order has fewer, larger tiles)
-    const int grid = (int)(tiles_ub < (unsigned)slots ? tiles_ub : (unsigned)slots);
-    kern<<<grid, msda::kTiledThreads, 0, st>>>(value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P, npairs,
-                                               allow_patches(), out);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-}
-
 // Launch of a backward kernel right after the grad_value zero-fill.  When msda_backward_* left t_pdl_next set, the fill
 // kernel just issued on `st` is the programmatic-dependent-launch primary: the backward kernel's prologue overlaps it and
 // the kernel waits for it (pdl_wait_primary) before its first red.
@@ -239,29 +200,65 @@ cudaError_t launch_after_fill(K kern, int grid, size_t smem, cudaStream_t st, Ar
     return cudaGetLastError();
 }
 
-template <typename T, int D, int LP_MAX, int VEC = BwdVec<T>::v, bool NORED = false>
-cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
-                       const float *attn, const Dims &d, float *gv, float *gl, float *ga, cudaStream_t st) {
-    constexpr int GPW = 32 / (D / VEC);
-    constexpr bool kCanStage = (LP_MAX <= 16);
-    constexpr bool kCanSplit = (LP_MAX % GPW == 0) && (LP_MAX / GPW <= D / VEC);
+// Persistent launch of a tiled kernel: one CTA per resident slot, but no more CTAs than the linear order has tiles (the
+// patch order has fewer, larger ones).  after_fill: the launch follows the grad_value zero-fill and honours the PDL
+// pairing with it (launch_after_fill); every other launch is a plain one and leaves t_pdl_next alone.
+template <typename K, typename... Args>
+cudaError_t launch_tiled(K kern, std::atomic<int> (&cache)[kMaxDevices], unsigned npairs, unsigned iter_pairs,
+                         bool after_fill, cudaStream_t st, Args... args) {
+    const unsigned slots = (unsigned)resident_ctas_cached(kern, cache);
+    const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;
+    const int grid = (int)(tiles_ub < slots ? tiles_ub : slots);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (after_fill) return launch_after_fill(kern, grid, 0, st, args...);
+    kern<<<grid, msda::kTiledThreads, 0, st>>>(args...);
+    return cudaGetLastError();
+}
+
+template <typename T, int D, int LP_MAX, int VEC = FwdVec<T>::v>
+cudaError_t launch_fwd(const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc, const float *attn,
+                       const Dims &d, T *out, cudaStream_t st) {
+    using Shape = msda::TiledShape<VEC, D, LP_MAX, false>;
+    constexpr bool kCanStage = (LP_MAX <= 16);          // per-warp double buffer must fit static shared memory
+    constexpr bool kCanSplit = Shape::kCanSplit;
+    constexpr bool kCanPack = sizeof(T) == 2 && VEC == 8;
     const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
     const bool split = kCanSplit && use_split(npairs);
     const bool tma = !split && kCanStage && use_tma_staging(d);
-    auto kern = split ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit, false, NORED>
-                : tma ? msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false, false, NORED>
-                      : msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>;
-    static std::atomic<int> c_split[kMaxDevices], c_tma[kMaxDevices], c_ldg[kMaxDevices];
-    const int slots = split ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit, false, NORED>, c_split)
-                      : tma ? resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false, false, NORED>, c_tma)
-                            : resident_ctas_cached(msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>, c_ldg);
-    const unsigned iter_pairs = msda::kTiledWarps * (split ? 1 : GPW);
-    const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;
-    const int grid = (int)(tiles_ub < (unsigned)slots ? tiles_ub : (unsigned)slots);
-    const cudaError_t e = launch_after_fill(kern, grid, 0, st, grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L,
-                                            d.Lq, d.P, npairs, allow_patches(), gv, gl, ga, (__nv_bfloat16 *)nullptr, 0);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return e;
+    // bf16: packed-bf16 corner blend for the large (non-split) launches
+    const bool packed = kCanPack && !split && knob(MSDA_KNOB_BF16_PACKED_FWD) == 1;
+    static decltype(&msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false>) const kern[] = {   // split, tma, ldg,
+        msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, kCanSplit>,                          // packed tma / ldg
+        msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, kCanStage, false>,
+        msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false>,
+        msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, kCanStage, false, kCanPack>,
+        msda::msda_fwd_tiled<T, VEC, D, LP_MAX, kFwdMinCtas, false, false, kCanPack>};
+    static std::atomic<int> cache[5][kMaxDevices];
+    const int k = split ? 0 : (packed ? 3 : 1) + (tma ? 0 : 1);
+    return launch_tiled(kern[k], cache[k], npairs, split ? msda::TiledShape<VEC, D, LP_MAX, kCanSplit>::kIterPairs
+                                                         : Shape::kIterPairs,
+                        false, st, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P, npairs, allow_patches(), out);
+}
+
+template <typename T, int D, int LP_MAX, int VEC = BwdVec<T>::v, bool NORED = false>
+cudaError_t launch_bwd(const T *grad_out, const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc,
+                       const float *attn, const Dims &d, float *gv, float *gl, float *ga, cudaStream_t st) {
+    using Shape = msda::TiledShape<VEC, D, LP_MAX, false>;
+    constexpr bool kCanStage = (LP_MAX <= 16);
+    constexpr bool kCanSplit = Shape::kCanSplit;
+    const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
+    const bool split = kCanSplit && use_split(npairs);
+    const bool tma = !split && kCanStage && use_tma_staging(d);
+    static decltype(&msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>) const kern[] = {
+        msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, kCanSplit, false, NORED>,          // split, tma, ldg
+        msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, kCanStage, false, false, NORED>,
+        msda::msda_bwd_tiled<T, VEC, D, LP_MAX, kBwdMinCtas, false, false, false, NORED>};
+    static std::atomic<int> cache[3][kMaxDevices];
+    const int k = split ? 0 : tma ? 1 : 2;
+    return launch_tiled(kern[k], cache[k], npairs, split ? msda::TiledShape<VEC, D, LP_MAX, kCanSplit>::kIterPairs
+                                                         : Shape::kIterPairs,
+                        true, st, grad_out, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P, npairs,
+                        allow_patches(), gv, gl, ga, (__nv_bfloat16 *)nullptr, 0);
 }
 
 // ---- slab-ordered kernels (msda_slab.cuh): D = 32 and L*P <= 16 (every UNINEXT call) ------------------------------
@@ -335,21 +332,15 @@ cudaError_t launch_bwd_mixed(const __nv_bfloat16 *go, const __nv_bfloat16 *value
                              float *gl, float *ga, int fine_min_rows, cudaStream_t st) {
     using T = __nv_bfloat16;
     constexpr int VEC = 4, DD = 32, LP_MAX = 16;
-    constexpr int GPW = 32 / (DD / VEC);
     const unsigned npairs = (unsigned)((long long)d.N * d.Lq * d.M);
-    const bool tma = use_tma_staging(d);
-    static std::atomic<int> c_tma[kMaxDevices], c_ldg[kMaxDevices];
-    auto k_tma = msda::msda_bwd_tiled<T, VEC, DD, LP_MAX, kBwdMinCtas, true, false, true>;
-    auto k_ldg = msda::msda_bwd_tiled<T, VEC, DD, LP_MAX, kBwdMinCtas, false, false, true>;
-    const int slots = tma ? resident_ctas_cached(k_tma, c_tma) : resident_ctas_cached(k_ldg, c_ldg);
-    const unsigned iter_pairs = msda::kTiledWarps * GPW;
-    const unsigned tiles_ub = (npairs + iter_pairs - 1) / iter_pairs;
-    const int grid = (int)(tiles_ub < (unsigned)slots ? tiles_ub : (unsigned)slots);
-    (tma ? k_tma : k_ldg)<<<grid, msda::kTiledThreads, 0, st>>>(go, value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq,
-                                                                 d.P, npairs, allow_patches(), scratch, gl, ga, gv16,
-                                                                 fine_min_rows);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
+    static decltype(&msda::msda_bwd_tiled<T, VEC, DD, LP_MAX, kBwdMinCtas, false, false, true>) const kern[] = {
+        msda::msda_bwd_tiled<T, VEC, DD, LP_MAX, kBwdMinCtas, true, false, true>,                     // tma, ldg
+        msda::msda_bwd_tiled<T, VEC, DD, LP_MAX, kBwdMinCtas, false, false, true>};
+    static std::atomic<int> cache[2][kMaxDevices];
+    const int k = use_tma_staging(d) ? 0 : 1;
+    return launch_tiled(kern[k], cache[k], npairs, msda::TiledShape<VEC, DD, LP_MAX, false>::kIterPairs, false, st, go,
+                        value, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P, npairs, allow_patches(), scratch,
+                        gl, ga, gv16, fine_min_rows);
 }
 
 // Backward with the coarse levels accumulated by dedicated consumer warps (msda_tmem.cuh): MSDA_KNOB_SLAB = 2.  The window
@@ -420,8 +411,8 @@ cudaError_t launch_bwd_region(const float *go, const float *value, const int64_t
     return e;
 }
 
-#define MSDA_ROUTE_LP(T, DD, CALL)                                   \
-    (LP <= 16 ? CALL<T, DD, 16> : CALL<T, DD, 32>)
+#define MSDA_ROUTE_LP(T, DD, CALL, ...)                              \
+    (LP <= 16 ? CALL<T, DD, 16, ##__VA_ARGS__> : CALL<T, DD, 32, ##__VA_ARGS__>)
 
 template <typename T>
 cudaError_t fwd_fast(const T *value, const int64_t *shapes, const int64_t *lsi, const float *loc, const float *attn,
@@ -541,17 +532,9 @@ cudaError_t det_loc_attn(const T *go, const T *value, const int64_t *shapes, con
         if (fast) {
             const int LP = d.L * d.P;
             switch (d.D) {
-                case 16:
-                    if constexpr (sizeof(T) == 4)
-                        return LP <= 16 ? launch_bwd<T, 16, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
-                                        : launch_bwd<T, 16, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
-                    break;
-                case 32:
-                    return LP <= 16 ? launch_bwd<T, 32, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
-                                    : launch_bwd<T, 32, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
-                case 64:
-                    return LP <= 16 ? launch_bwd<T, 64, 16, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st)
-                                    : launch_bwd<T, 64, 32, 4, true>(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+                case 16: if constexpr (sizeof(T) == 4) return MSDA_ROUTE_LP(T, 16, launch_bwd, 4, true)(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st); break;
+                case 32: return MSDA_ROUTE_LP(T, 32, launch_bwd, 4, true)(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
+                case 64: return MSDA_ROUTE_LP(T, 64, launch_bwd, 4, true)(go, value, shapes, lsi, loc, attn, d, gv, gl, ga, st);
             }
             return cudaErrorInvalidValue;
         }
