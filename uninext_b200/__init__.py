@@ -2,7 +2,8 @@
 transformer, behind the reference's own operator boundary.
 
 Layout
-    csrc/        hand-written CUDA kernels + the C ABI (include/msda_b200.h)  -> lib/libmsda_b200.so
+    csrc/        hand-written CUDA kernels + the C ABI (include/msda_b200.h), one msda_cabi*.cu per kernel family
+                 -> lib/libmsda_b200.so
     _cabi.py     ctypes binding (fails loudly when the library is missing; there is no fallback)
     dropin/      ``MultiScaleDeformableAttention`` -- module-level drop-in for the reference's pybind extension
     functions/   ``MSDeformAttnFunction`` (reference autograd signature) and a bf16 variant

@@ -12,6 +12,7 @@ import os
 import shutil
 import subprocess
 import sys
+from concurrent.futures import ThreadPoolExecutor
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
@@ -19,13 +20,14 @@ LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmsda_b200.so")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 
-SOURCES = ["msda_cabi.cu", "msda_gemm_sm90.cu"]
-HEADERS = ["msda_common.cuh", "msda_tiled.cuh", "msda_region.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh", "msda_maskpaste.cuh", "msda_maskrle.cuh","msda_detpost.cuh", "msda_det.cuh", "msda_vlfuse.cuh", "msda_vlfuse_tc.cuh"]
+SOURCES = ["msda_cabi.cu", "msda_cabi_module.cu", "msda_cabi_condinst.cu", "msda_cabi_postprocess.cu", "msda_cabi_vlfuse.cu",
+           "msda_gemm_sm90.cu"]
+HEADERS = ["msda_host.cuh", "msda_common.cuh", "msda_tiled.cuh", "msda_region.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh", "msda_maskpaste.cuh", "msda_maskrle.cuh","msda_detpost.cuh", "msda_det.cuh", "msda_vlfuse.cuh", "msda_vlfuse_tc.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
-    "--shared", "-Xcompiler", "-fPIC",
+    "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
     "--expt-relaxed-constexpr",
 ]
@@ -52,12 +54,20 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
     tmp = f"{LIB_PATH}.tmp.{os.getpid()}"          # link under a private name, then rename: readers never see a partial file
-    cmd = [nvcc_path()] + NVCC_FLAGS + ["-I", INCLUDE, "-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    log = proc.stdout + proc.stderr
+    objs = [f"{tmp}.{os.path.splitext(s)[0]}.o" for s in SOURCES]
+    cmds = [[nvcc_path()] + NVCC_FLAGS + ["-I", INCLUDE, "-c", os.path.join(CSRC, s), "-o", o] for s, o in zip(SOURCES, objs)]
+    with ThreadPoolExecutor(len(cmds)) as pool:    # one translation unit per kernel family, compiled concurrently
+        procs = list(pool.map(lambda c: subprocess.run(c, capture_output=True, text=True), cmds))
+    if all(p.returncode == 0 for p in procs):
+        cmds.append([nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "--shared", "-o", tmp] + objs)
+        procs.append(subprocess.run(cmds[-1], capture_output=True, text=True))
+    log = "".join(" ".join(c) + "\n" + p.stdout + p.stderr for c, p in zip(cmds, procs))
     with open(os.path.join(LIB_DIR, "build.log"), "w") as fh:
-        fh.write(" ".join(cmd) + "\n" + log)
-    if proc.returncode != 0:
+        fh.write(log)
+    for o in objs:
+        if os.path.exists(o):
+            os.remove(o)
+    if any(p.returncode != 0 for p in procs):      # a failed compile is never linked
         sys.stderr.write(log)
         if os.path.exists(tmp):
             os.remove(tmp)

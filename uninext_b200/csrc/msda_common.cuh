@@ -18,22 +18,12 @@ constexpr unsigned kFullMask = 0xffffffffu;
 
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------------------
 // grad_value must be zero before the backward kernel's first red.  With MSDA_KNOB_ZERO_FILL = 2 the zero-fill kernel
-// below and the backward kernel are a PDL pair: the fill kernel lets its dependent launch as soon as all of its CTAs are
-// running, the backward kernel builds its work map, initialises its mbarriers and starts its first TMA tap loads (none
-// of which touch grad_value), and only then waits for the fill to have completed and flushed.  Without the launch
-// attribute both instructions are no-ops.
+// (msda_zero_fill, msda_generic.cuh) and the backward kernel are a PDL pair: the fill kernel lets its dependent launch
+// as soon as all of its CTAs are running, the backward kernel builds its work map, initialises its mbarriers and starts
+// its first TMA tap loads (none of which touch grad_value), and only then waits for the fill to have completed and
+// flushed.  Without the launch attribute both instructions are no-ops.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait_primary() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-// Zero-fill of a 16-byte aligned buffer of n16 x 16 bytes: one wave of CTAs, 16-byte stores, grid stride.
-__global__ void __launch_bounds__(256) msda_zero_fill(uint4 *__restrict__ p, unsigned long long n16) {
-    pdl_launch_dependents();
-    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
-    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-#pragma unroll 4
-    for (; i < n16; i += stride) p[i] = z;
-}
 
 // Geometry of one bilinear tap, resolved against one level map.
 //   r0 / r1 : row index (within one batch element, i.e. in [0, S)) of the clamped (h0, w0) / (h1, w0) corners.

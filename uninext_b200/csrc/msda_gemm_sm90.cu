@@ -17,13 +17,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <atomic>
 #include <mutex>
 
 #include "../../include/msda_b200.h"
-
-extern std::atomic<uint64_t> g_msda_gemm_launches;
-std::atomic<uint64_t> g_msda_gemm_launches{0};
+#include "msda_host.cuh"
 
 namespace gemm {
 
@@ -261,22 +258,11 @@ int launch(const float *A, const float *W, const float *bias, const unsigned cha
     Params p;
     p.M = M; p.N = N; p.K = K; p.stages = stages; p.relu = relu; p.bias = bias; p.row_mask = row_mask; p.C = C;
     const size_t smem = (size_t)stages * stage_bytes + 1024;
-    // function attributes and SM counts are per DEVICE: cache them per ordinal (a process may drive several GPUs)
-    constexpr int kMaxDev = 64;
-    static std::atomic<int> sms_of[kMaxDev];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDev) dev = 0;
-    int sms = sms_of[dev].load(std::memory_order_relaxed);
-    if (sms == 0) {
-        const cudaError_t e = cudaFuncSetAttribute(linear_tf32_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max);
-        if (e != cudaSuccess) return (int)e;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-        sms_of[dev].store(sms, std::memory_order_relaxed);
-    }
+    if (const cudaError_t e = msda_host::opt_in_smem<linear_tf32_kernel<BN>>((int)dyn_max)) return (int)e;
+    const int sms = msda_host::num_sms();
     const long long tiles = (M + BLOCK_M - 1) / BLOCK_M * (N / BN);
     const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-    linear_tf32_kernel<BN><<<grid, kThreads, smem, stream>>>(map_a, map_w, p);
-    g_msda_gemm_launches.fetch_add(1, std::memory_order_relaxed);
+    linear_tf32_kernel<BN><<<grid, kThreads, smem, stream>>>(map_a, map_w, p);    // not counted by msda_launch_count()
     return (int)cudaGetLastError();
 }
 

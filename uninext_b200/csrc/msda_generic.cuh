@@ -150,6 +150,16 @@ msda_bwd_generic(const T *__restrict__ grad_out, const T *__restrict__ value,
     }
 }
 
+// Zero-fill of a 16-byte aligned buffer of n16 x 16 bytes: one wave of CTAs, 16-byte stores, grid stride.
+__global__ void __launch_bounds__(256) msda_zero_fill(uint4 *__restrict__ p, unsigned long long n16) {
+    pdl_launch_dependents();
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+#pragma unroll 4
+    for (; i < n16; i += stride) p[i] = z;
+}
+
 // fp32 accumulator -> bf16 result (bf16 backward only)
 __global__ void __launch_bounds__(256)
 msda_f32_to_bf16(const float *__restrict__ src, __nv_bfloat16 *__restrict__ dst, long long n) {
