@@ -67,6 +67,18 @@ SIGNATURES = {
     "msda_vlfuse_backward_bf16": (_i, [_vp] * 10 + [_i] * 7 + [ctypes.c_float, _vp] + [_vp] * 5 + [ctypes.c_int64, _vp]),
 }
 ABI_VERSION = 11
+
+# The two-stage query selection's entry points (include/msda_twostage.h), typed by load() when the library exports them;
+# twostage() raises MSDALibraryError for a library that does not.
+_i64 = ctypes.c_int64
+TWOSTAGE_SIGNATURES = {
+    "msda_twostage_head_forward_f32": (_i, [_vp] * 7 + [_i] * 3 + [ctypes.c_float, _i] + [_vp] * 4 + [_vp]),
+    "msda_twostage_head_workspace": (_i, [_i] * 3 + [_vp]),
+    "msda_twostage_head_backward_f32": (_i, [_vp] * 11 + [_i] * 4 + [_vp] * 6 + [_vp, _i64, _vp]),
+    "msda_twostage_select_workspace": (_i, [_i] * 3 + [_vp]),
+    "msda_twostage_select_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_vp, _i64, _vp]),
+    "msda_twostage_select_backward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp]),
+}
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 
@@ -97,10 +109,24 @@ def load(path: str | None = None):
         except AttributeError as exc:
             raise MSDALibraryError(f"{p} does not export `{name}` (stale build? run uninext_b200.build --force)") from exc
         fn.restype, fn.argtypes = res, args
+    lib.twostage_missing = [name for name in TWOSTAGE_SIGNATURES if not hasattr(lib, name)]
+    for name, (res, args) in TWOSTAGE_SIGNATURES.items():
+        if name not in lib.twostage_missing:
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = res, args
     if lib.msda_abi_version() != ABI_VERSION:
         raise MSDALibraryError(f"{p}: ABI version {lib.msda_abi_version()} != expected {ABI_VERSION}")
     if path is None:
         _lib = lib
+    return lib
+
+
+def twostage(path: str | None = None):
+    """The loaded library, after checking that it exports the two-stage selection (include/msda_twostage.h)."""
+    lib = load(path)
+    if lib.twostage_missing:
+        raise MSDALibraryError(f"{path or LIB_PATH} does not export `{lib.twostage_missing[0]}` (stale build? run "
+                               "uninext_b200.build --force)")
     return lib
 
 

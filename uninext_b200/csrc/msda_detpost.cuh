@@ -18,6 +18,7 @@
 #pragma once
 
 #include "msda_common.cuh"
+#include "msda_topk.cuh"
 
 namespace msda {
 
@@ -85,14 +86,6 @@ __device__ __forceinline__ bool dp_iou_above(float4 a, float4 b, float thr) {
     const float sa = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
     const float sb = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
     return __fdiv_rn(inter, __fsub_rn(__fadd_rn(sa, sb), inter)) > thr;
-}
-
-// The sort key of a candidate: descending value in the high word, ascending flat index (kept rank * C + class) in the
-// low word.  Unique per candidate, so "the count smallest keys" is exactly the top-k in the documented order.
-__device__ __forceinline__ unsigned long long dp_key(float v, unsigned flat) {
-    unsigned u = __float_as_uint(v);
-    u ^= (u >> 31) ? 0xffffffffu : 0x80000000u;             // ascending unsigned order = ascending float order
-    return ((unsigned long long)(~u) << 32) | flat;
 }
 
 __device__ __forceinline__ float dp_block_max(float v, float *red) {
@@ -193,33 +186,8 @@ detpost_select(const float *__restrict__ box_pred, const int *__restrict__ image
         const int qi = NMS ? s_keep[r] : (int)r;
         return dp_key(pr[(size_t)qi * C + c], f);
     };
-    // radix select of the cnt-th smallest key, 8 bits at a time from the top; stops once the chosen bucket is taken whole
-    unsigned long long prefix = 0, pmask = 0, thr = ~0ull;
-    unsigned remaining = cnt;
-    for (int shift = 56; shift >= 0; shift -= 8) {
-        for (int d = tid; d < 256; d += kDpThreads) s_hist[d] = 0;
-        __syncthreads();
-        for (unsigned f = tid; f < N; f += kDpThreads) {
-            const unsigned long long k = key_of(f);
-            if ((k & pmask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255], 1u);
-        }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned cum = 0;
-            for (int d = 0; d < 256; ++d) {
-                const unsigned h = s_hist[d];
-                if (cum + h >= remaining) { s_digit = d; s_rem = remaining - cum; s_bucket = h; break; }
-                cum += h;
-            }
-        }
-        __syncthreads();
-        prefix |= (unsigned long long)s_digit << shift;
-        pmask |= 0xffull << shift;
-        remaining = s_rem;
-        const bool whole = s_bucket == remaining;
-        __syncthreads();                        // s_digit / s_rem / s_bucket are rewritten by the next pass
-        if (whole) { thr = prefix | ~pmask; break; }
-    }
+    // the cnt-th smallest key; the candidate keys are unique (flat index in the low word), so exactly cnt are <= thr
+    const unsigned long long thr = block_radix_threshold<kDpThreads>(N, cnt, key_of, s_hist, &s_digit, &s_rem, &s_bucket);
     // collect the cnt keys <= thr (in any order), pad to a power of two, bitonic sort ascending
     unsigned P = 1;
     while (P < cnt) P <<= 1;
@@ -232,18 +200,7 @@ detpost_select(const float *__restrict__ box_pred, const int *__restrict__ image
     }
     for (unsigned i = cnt + tid; i < P; i += kDpThreads) buf[i] = ~0ull;
     __syncthreads();
-    for (unsigned k = 2; k <= P; k <<= 1) {
-        for (unsigned j = k >> 1; j > 0; j >>= 1) {
-            for (unsigned i = tid; i < P; i += kDpThreads) {
-                const unsigned ixj = i ^ j;
-                if (ixj > i) {
-                    const unsigned long long x = buf[i], y = buf[ixj];
-                    if ((x > y) == ((i & k) == 0)) { buf[i] = y; buf[ixj] = x; }
-                }
-            }
-            __syncthreads();
-        }
-    }
+    block_bitonic_sort<kDpThreads>(buf, P);
     // outputs: boxes xyxy then Boxes.scale (x * w, y * h); entries past cnt get the fill values
     const float sh = (float)image_sizes[2 * b], sw = (float)image_sizes[2 * b + 1];
     const size_t o = (size_t)b * max_inst;

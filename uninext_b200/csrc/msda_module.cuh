@@ -3,11 +3,13 @@
 //     written directly in the op's layouts (reference: ops/modules/ms_deform_attn.py:99-112, five elementwise passes);
 //   * its backward (softmax backward + location scaling) producing the gradient of the raw projection;
 //   * column sums (bias gradients of the bracketing Linears);
-//   * residual-add + LayerNorm forward / backward (deformable_transformer.py:354-356,359 `norm(src + dropout(x))`).
+//   * residual-add + LayerNorm forward / backward (deformable_transformer.py:354-356,359 `norm(src + dropout(x))`), on the
+//     row code of msda_layernorm.cuh.
 // All fp32; every kernel is one pass over its operands.
 #pragma once
 
 #include "msda_common.cuh"
+#include "msda_layernorm.cuh"
 
 namespace msda {
 
@@ -15,12 +17,6 @@ template <int G>
 __device__ __forceinline__ float group_max(float v) {
 #pragma unroll
     for (int d = G / 2; d >= 1; d >>= 1) v = fmaxf(v, __shfl_xor_sync(kFullMask, v, d, G));
-    return v;
-}
-template <int G>
-__device__ __forceinline__ float group_sum(float v) {
-#pragma unroll
-    for (int d = G / 2; d >= 1; d >>= 1) v += __shfl_xor_sync(kFullMask, v, d, G);
     return v;
 }
 
@@ -306,27 +302,20 @@ msda_add_layernorm_fwd(const float *__restrict__ a, const float *__restrict__ b,
         }
         s += v[i].x + v[i].y + v[i].z + v[i].w;
     }
-    const float mu = group_sum<32>(s) * (1.f / C);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < V; ++i) {
-        const float dx = v[i].x - mu, dy = v[i].y - mu, dz = v[i].z - mu, dw = v[i].w - mu;
-        q += dx * dx + dy * dy + dz * dz + dw * dw;
-    }
-    const float rs = rsqrtf(group_sum<32>(q) * (1.f / C) + eps);
+    float mu, rs;
+    ln_row_stats<V>(v, s, eps, mu, rs);
 #pragma unroll
     for (int i = 0; i < V; ++i) {
         const long long o = row * (C / 4) + i * 32 + lane;
         const float4 g = __ldg(reinterpret_cast<const float4 *>(gamma) + i * 32 + lane);
         const float4 bt = __ldg(reinterpret_cast<const float4 *>(beta) + i * 32 + lane);
         if (z != nullptr) reinterpret_cast<float4 *>(z)[o] = v[i];
-        reinterpret_cast<float4 *>(y)[o] = make_float4((v[i].x - mu) * rs * g.x + bt.x, (v[i].y - mu) * rs * g.y + bt.y,
-                                                       (v[i].z - mu) * rs * g.z + bt.z, (v[i].w - mu) * rs * g.w + bt.w);
+        reinterpret_cast<float4 *>(y)[o] = ln_affine(v[i], mu, rs, g, bt);
     }
     if (lane == 0) { mean[row] = mu; rstd[row] = rs; }
 }
 
-// dz = rstd * (dy*gamma - mean(dy*gamma) - xhat * mean(dy*gamma*xhat));  dgamma += sum_rows dy*xhat;  dbeta += sum_rows dy.
+// dz (ln_row_bwd);  dgamma += sum_rows dy*xhat;  dbeta += sum_rows dy.
 // Each warp walks rows warp, warp+W, ...; its per-lane column partials are combined across the CTA's warps in shared
 // memory and leave the CTA as one 16-byte red per lane-slice.  dgamma / dbeta must be zero on entry.
 template <int V>
@@ -347,8 +336,7 @@ msda_layernorm_bwd(const float *__restrict__ dy, const float *__restrict__ z, co
     }
     for (long long row = r0 + warp; row < r1; row += 8) {
         const float mu = __ldg(mean + row), rs = __ldg(rstd + row);
-        float4 d[V], xh[V];
-        float s1 = 0.f, s2 = 0.f;
+        float4 d[V], xh[V], dzr[V];
 #pragma unroll
         for (int i = 0; i < V; ++i) {
             const long long o = row * (C / 4) + i * 32 + lane;
@@ -357,18 +345,10 @@ msda_layernorm_bwd(const float *__restrict__ dy, const float *__restrict__ z, co
             xh[i] = make_float4((zz.x - mu) * rs, (zz.y - mu) * rs, (zz.z - mu) * rs, (zz.w - mu) * rs);
             ab[i].x += d[i].x; ab[i].y += d[i].y; ab[i].z += d[i].z; ab[i].w += d[i].w;
             ag[i].x += d[i].x * xh[i].x; ag[i].y += d[i].y * xh[i].y; ag[i].z += d[i].z * xh[i].z; ag[i].w += d[i].w * xh[i].w;
-            d[i].x *= g[i].x; d[i].y *= g[i].y; d[i].z *= g[i].z; d[i].w *= g[i].w;       // dy * gamma
-            s1 += d[i].x + d[i].y + d[i].z + d[i].w;
-            s2 += d[i].x * xh[i].x + d[i].y * xh[i].y + d[i].z * xh[i].z + d[i].w * xh[i].w;
         }
-        s1 = group_sum<32>(s1) * (1.f / C);
-        s2 = group_sum<32>(s2) * (1.f / C);
+        ln_row_bwd<V>(d, xh, g, rs, dzr);
 #pragma unroll
-        for (int i = 0; i < V; ++i) {
-            const long long o = row * (C / 4) + i * 32 + lane;
-            reinterpret_cast<float4 *>(dz)[o] = make_float4(rs * (d[i].x - s1 - xh[i].x * s2), rs * (d[i].y - s1 - xh[i].y * s2),
-                                                            rs * (d[i].z - s1 - xh[i].z * s2), rs * (d[i].w - s1 - xh[i].w * s2));
-        }
+        for (int i = 0; i < V; ++i) reinterpret_cast<float4 *>(dz)[row * (C / 4) + i * 32 + lane] = dzr[i];
     }
 #pragma unroll
     for (int i = 0; i < V; ++i) { sg[warp][i * 32 + lane] = ag[i]; sb[warp][i * 32 + lane] = ab[i]; }
