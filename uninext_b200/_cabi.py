@@ -79,6 +79,12 @@ TWOSTAGE_SIGNATURES = {
     "msda_twostage_select_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_vp, _i64, _vp]),
     "msda_twostage_select_backward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp]),
 }
+# The encoder's input preparation (include/msda_flatten.h), loaded the same way; flatten() raises for a library without.
+FLATTEN_SIGNATURES = {
+    "msda_flatten_levels_forward_f32": (_i, [_vp] * 5 + [_i] * 3 + [_vp] * 4 + [_vp]),
+    "msda_flatten_levels_workspace": (_i, [_vp] * 2 + [_i] * 3 + [_vp]),
+    "msda_flatten_levels_backward_f32": (_i, [_vp] * 4 + [_i] * 3 + [_vp] * 4 + [_i64, _vp]),
+}
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 
@@ -110,8 +116,9 @@ def load(path: str | None = None):
             raise MSDALibraryError(f"{p} does not export `{name}` (stale build? run uninext_b200.build --force)") from exc
         fn.restype, fn.argtypes = res, args
     lib.twostage_missing = [name for name in TWOSTAGE_SIGNATURES if not hasattr(lib, name)]
-    for name, (res, args) in TWOSTAGE_SIGNATURES.items():
-        if name not in lib.twostage_missing:
+    lib.flatten_missing = [name for name in FLATTEN_SIGNATURES if not hasattr(lib, name)]
+    for name, (res, args) in list(TWOSTAGE_SIGNATURES.items()) + list(FLATTEN_SIGNATURES.items()):
+        if hasattr(lib, name):
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = res, args
     if lib.msda_abi_version() != ABI_VERSION:
@@ -126,6 +133,15 @@ def twostage(path: str | None = None):
     lib = load(path)
     if lib.twostage_missing:
         raise MSDALibraryError(f"{path or LIB_PATH} does not export `{lib.twostage_missing[0]}` (stale build? run "
+                               "uninext_b200.build --force)")
+    return lib
+
+
+def flatten(path: str | None = None):
+    """The loaded library, after checking that it exports the input preparation (include/msda_flatten.h)."""
+    lib = load(path)
+    if lib.flatten_missing:
+        raise MSDALibraryError(f"{path or LIB_PATH} does not export `{lib.flatten_missing[0]}` (stale build? run "
                                "uninext_b200.build --force)")
     return lib
 
