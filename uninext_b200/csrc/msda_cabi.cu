@@ -143,9 +143,10 @@ constexpr int kFwdMinCtas = 4, kBwdMinCtas = 2;     // r01d sweep: fwd flat for 
 template <typename T> struct FwdVec { static constexpr int v = 16 / sizeof(T); };      // 16-byte row slices
 template <typename T> struct BwdVec { static constexpr int v = 4; };                  // 4 channels per lane (see RowVec)
 
-// Launch of a kernel of kTiledThreads threads.  pdl: the grad_value zero-fill kernel just issued on `st` is the
-// programmatic-dependent-launch primary (zero_fill reported it): the kernel's prologue overlaps the fill, and the kernel
-// must wait for it (pdl_wait_primary) before touching grad_value.  Only the backward kernels that do so take `pdl`.
+// Launch of a kernel of kTiledThreads threads.  pdl: the kernel just issued on `st` is the programmatic-dependent-launch
+// primary (the grad_value zero-fill, as zero_fill reported it, or the region backward's tap kernel): the kernel's
+// prologue overlaps the primary, and the kernel must wait for it (pdl_wait_primary) before touching grad_value.  Only the
+// backward kernels that do so take `pdl`.
 template <typename K, typename... Args>
 cudaError_t launch_after_fill(K kern, int grid, size_t smem, cudaStream_t st, bool pdl, Args... args) {
     if (pdl) {
@@ -330,24 +331,35 @@ bool use_region(const Dims &d) {
            !use_split(num_pairs(d));
 }
 
+// Two launches: the tap kernel (grad_loc / grad_attn), a PDL secondary of the zero-fill when `pdl`, then the grad_value
+// kernel, a PDL secondary of the tap kernel whenever the stream is not capturing (msda_region.cuh: the chain is
+// transitive).  Under capture the grad_value kernel follows in plain stream order.
 cudaError_t launch_bwd_region(const float *go, const float *value, const int64_t *shapes, const int64_t *lsi,
                               const float *loc, const float *attn, const Dims &d, float *gv, float *gl, float *ga,
                               bool pdl, cudaStream_t st) {
-    constexpr auto kern = msda::msda_bwd_region<msda::kRegionEdge, msda::kRegionHalo>;
-    constexpr size_t smem = msda::region_smem_bytes();
-    if (const cudaError_t e = opt_in_smem<kern>((int)smem)) return e;
-    static PerDevice<int> slots_c;
-    const int slots = slots_c.get([&](int) {
+    constexpr auto tap = msda::msda_bwd_region<msda::kRegionEdge, msda::kRegionHalo>;
+    constexpr auto gvk = msda::msda_region_grad_value_pass<msda::kRegionEdge, msda::kRegionHalo>;
+    constexpr size_t tap_smem = msda::region_tap_smem_bytes(), gv_smem = msda::region_gv_smem_bytes();
+    if (const cudaError_t e = opt_in_smem<gvk>((int)gv_smem)) return e;
+    const auto resident = [](auto kern, size_t smem) {
         int per_sm = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, msda::kTiledThreads, smem) != cudaSuccess || per_sm < 1)
             per_sm = 1;
         return per_sm * num_sms();
-    });
+    };
+    static PerDevice<int> tap_slots, gv_slots;
+    const int tap_grid = tap_slots.get([&](int) { return resident(tap, tap_smem); });
+    const int gv_grid = gv_slots.get([&](int) { return resident(gvk, gv_smem); });
+    const unsigned npairs = num_pairs(d);
     const int tma = use_tma_staging(d) ? 1 : 0;            // the tap pass: TMA-staged or __ldg taps, as msda_bwd_tiled
-    const cudaError_t e = launch_after_fill(kern, slots, smem, st, pdl, go, value, shapes, lsi, loc, attn, d.N, d.S, d.M,
-                                            d.L, d.Lq, d.P, num_pairs(d), tma, gv, gl, ga);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return e;
+    g_launches.fetch_add(2, std::memory_order_relaxed);
+    cudaError_t e = launch_after_fill(tap, tap_grid, tap_smem, st, pdl, go, value, shapes, lsi, loc, attn, d.N, d.S, d.M,
+                                      d.L, d.Lq, d.P, npairs, tma, gl, ga);
+    if (e != cudaSuccess) return e;
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    const bool chain = cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
+    return launch_after_fill(gvk, gv_grid, gv_smem, st, chain, go, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P,
+                             npairs, gv);
 }
 
 template <typename T>

@@ -7,22 +7,26 @@
 // queries of one (batch, head) whose pixel centre lies in one R x R region of the finest level touches only a small
 // rectangle ("window") of each level, and it can add those contributions up on chip first.
 //
-// grad_value's sums need each tap's geometry and the pair's grad_out, never `value`.  So one launch runs two passes in
-// every CTA, one after the other:
-//   tap pass: msda_bwd_tiled's NORED body (linear chunks of pairs, taps TMA-staged one iteration ahead when L*P % 4 == 0):
-//             the gathers, grad_loc and grad_attn, from the same device code and in the same FMA order as msda_bwd_tiled.
-//   grad_value pass, per tile = (b, m, region).  A query at pixel (x, y) of level l belongs to region
-//             floor((x + 0.5) * Wref / W_l / R) in x (likewise in y; Wref / Href = the largest level), so a region holds
-//             one contiguous x-range and y-range per level, in closed form.  The window on level l is the region scaled to
-//             level l plus kRegionHalo pixels.
+// grad_value's sums need each tap's geometry and the pair's grad_out, never `value`, and nothing of grad_loc /
+// grad_attn.  So the backward is two kernels, each with its own register and shared-memory budget:
+//   msda_bwd_region (tap pass, 2 CTAs/SM): msda_bwd_tiled's NORED body (linear chunks of pairs, taps TMA-staged one
+//             iteration ahead when L*P % 4 == 0): the gathers, grad_loc and grad_attn, from the same device code and in
+//             the same FMA order as msda_bwd_tiled.
+//   msda_region_grad_value_pass (3 CTAs/SM), per tile = (b, m, region).  A query at pixel (x, y) of level l belongs to
+//             region floor((x + 0.5) * Wref / W_l / R) in x (likewise in y; Wref / Href = the largest level), so a
+//             region holds one contiguous x-range and y-range per level, in closed form.  The window on level l is the
+//             region scaled to level l plus kRegionHalo pixels.
 //     phase A: one 8-lane group per pair; the lane that resolves a tap files its non-zero in-window corners as entries
 //              {window row, coefficient} at the fixed positions (slot, tap, corner) and counts each for its window row with
 //              a non-returning shared atomic.  The pair's grad_out row is stashed in shared memory.  A corner outside the
 //              window, or of a query past the stash, reds directly as in msda_bwd_tiled (its weight and rows go through
 //              the group's tap slab), so the capacities never change a result.  No value row is read.
-//     phase B: scan of the row counts, then scatter of the entries by window row (integer shared atomics only: fp32 shared
-//              atomics are CAS loops) into {coefficient, slot} arrays.
+//     phase B: scan of the row counts, then scatter of the entry indices by window row (integer shared atomics only:
+//              fp32 shared atomics are CAS loops) into one u16 array.
 //     phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
+// PDL chain: zero-fill (primary) -> tap kernel -> grad_value kernel.  The tap kernel writes nothing the fill writes, so it
+// lets its dependent launch at once and waits for the fill as its last statement: its completion then implies the fill's,
+// and the grad_value kernel, which waits for the tap kernel before its first red, sees a zeroed grad_value.
 // A level table that does not tile [0, S) (the patch-order condition) runs the grad_value pass in linear chunks of pairs
 // with no window: every corner reds directly.
 #pragma once
@@ -39,28 +43,30 @@ constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past t
 // (tests/region_layout.py) reads it.
 constexpr int kRegionStageRows = 384;
 constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
-constexpr int kRegionMinCtas = 2;
+constexpr int kRegionTapCtas = 2;         // tap kernel: it needs 128 registers per thread
+constexpr int kRegionGvCtas = 3;          // grad_value kernel: latency-bound, so as many resident warps as fit
 constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
 
-// The tap pass's TMA stage buffers (kTiledWarps per-warp double buffers of one iteration's (x, y, a)).
+// The tap kernel's TMA stage buffers (kTiledWarps per-warp double buffers of one iteration's (x, y, a)).
 using RegionTapStage = TapStage<4, 16, true>;
 
-// Dynamic shared memory: entry coefficients (f32) + grad_out stash + row counts + entry rows (u16) + the sorted
-// {coefficient (f32), slot (u8)} arrays.  The tap pass's stage buffers overlay the entry coefficients: the passes run
-// one after the other.
-constexpr size_t region_smem_bytes() {
-    static_assert((size_t)kTiledWarps * RegionTapStage::kBytes <= (size_t)kRegionEntries * 4, "stage buffers overlay e_coef");
-    return (size_t)kRegionEntries * (4 + 2) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4 +
-           (size_t)kRegionEntries * (4 + 1);
+// Dynamic shared memory of the tap kernel: its stage buffers.
+constexpr size_t region_tap_smem_bytes() { return (size_t)kTiledWarps * RegionTapStage::kBytes; }
+
+// Dynamic shared memory of the grad_value kernel: entry coefficients (f32) + grad_out stash + row counts + entry rows
+// (u16) + the entry indices sorted by window row (u16).
+constexpr size_t region_gv_smem_bytes() {
+    static_assert(kRegionEntries <= 0x10000, "entry indices are u16");
+    return (size_t)kRegionEntries * (4 + 2 + 2) + (size_t)kRegionSlots * 128 + (size_t)kRegionWinRows * 4;
 }
 
 #ifdef MSDA_REGION_PHASE_CLOCKS
-// Timing hook for tools/region_phases.py; the library build never defines it.  Thread 0 of each CTA adds the clock64()
-// span since the previous stamp into g_region_clocks[blockIdx.x * kRegionSpans + span], after a CTA barrier: span 0 = tap
-// pass, 1 = tile geometry + count reset, 2 = phase A, 3 = phase B, 4 = phase C.  g_region_knockout bit 0 drops phase A's
+// Timing hook for tools/region_phases.py; the library build never defines it.  Thread 0 of each grad_value CTA adds the
+// clock64() span since the previous stamp into g_region_clocks[blockIdx.x * kRegionSpans + span], after a CTA barrier:
+// span 0 = tile geometry + count reset, 1 = phase A, 2 = phase B, 3 = phase C.  g_region_knockout bit 0 drops phase A's
 // direct reds, bit 1 phase C's (the sums are still formed); results are then wrong by construction and serve only for
 // timing.
-constexpr int kRegionSpans = 5;
+constexpr int kRegionSpans = 4;
 __device__ unsigned long long *g_region_clocks;
 __device__ int g_region_knockout;
 #define MSDA_REGION_CLOCK_INIT long long region_clk = clock64()
@@ -97,14 +103,15 @@ __device__ __forceinline__ int region_first(int r, int n, int ref, int R) {
     return num <= 0 ? 0 : (int)min((long long)n, (num + 2ll * ref - 1) / (2ll * ref));
 }
 
-// The grad_value pass.  It is a separate function, called once per CTA, so that nothing it computes is hoisted into the
-// tap pass: the tap pass needs the kernel's whole 128-register budget (2 CTAs/SM), and any value of this pass kept live
-// through it is a spill.
+// The grad_value pass, a persistent PDL secondary of the tap kernel (msda_bwd_region).  Its first tile's geometry and
+// entries overlap the tap kernel's last wave; it waits for the tap kernel, and through it for the zero-fill, before its
+// first red.
 template <int R, int HALO>
-__device__ __noinline__ void
-region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__restrict__ shapes,
-                       const int64_t *__restrict__ lsi, const float *__restrict__ loc, const float *__restrict__ attn,
-                       int N, int S, int M, int L, int Lq, int P, unsigned npairs, float *__restrict__ grad_value)
+__global__ void __launch_bounds__(kTiledThreads, kRegionGvCtas)
+msda_region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__restrict__ shapes,
+                            const int64_t *__restrict__ lsi, const float *__restrict__ loc,
+                            const float *__restrict__ attn, int N, int S, int M, int L, int Lq, int P, unsigned npairs,
+                            float *__restrict__ grad_value)
 {
     constexpr int D = 32, VEC = 4, LPR = D / VEC, GPW = 32 / LPR, LP_MAX = 16, NSL = LP_MAX / LPR;
     static_assert(GPW * kTiledWarps == kRegionIterSlots && kRegionSlots <= 256 && kRegionWinRows < 0xffff &&
@@ -120,8 +127,7 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
     float4 *gstash = reinterpret_cast<float4 *>(e_coef + kRegionEntries);             // [slot][lane] grad_out slices
     int *cnt = reinterpret_cast<int *>(gstash + kRegionSlots * LPR);                  // [window row]
     unsigned short *e_row = reinterpret_cast<unsigned short *>(cnt + kRegionWinRows); // [slot][tap][corner], kNoRow = none
-    float *s_coef = reinterpret_cast<float *>(e_row + kRegionEntries);                // phases B, C: sorted by window row
-    unsigned char *s_slot = reinterpret_cast<unsigned char *>(s_coef + kRegionEntries);
+    unsigned short *s_idx = e_row + kRegionEntries;     // phases B, C: entry indices sorted by window row
 
     MSDA_REGION_CLOCK_INIT;
     if (threadIdx.x == 0) {            // the map comes from the device-resident level table: no host read, capture-safe
@@ -148,6 +154,7 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
     const int LP = L * P;
     const unsigned row_elems = (unsigned)(M * D);
     TapSlab<LPR> slab(slab_mem + warp * TapSlab<LPR>::kBytes, grp);
+    bool primary_done = false;         // CTA-uniform: pdl_wait_primary() has returned
     for (unsigned tile = blockIdx.x; tile < rm.ntiles; tile += gridDim.x) {
         // ---- tile geometry: thread l resolves level l, thread 0 then lays the levels out ----
         if (rm.region) {
@@ -187,7 +194,7 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
         __syncthreads();
         for (int i = threadIdx.x; i < tl.nwin; i += kTiledThreads) cnt[i] = 0;
         __syncthreads();
-        MSDA_REGION_CLOCK(1);
+        MSDA_REGION_CLOCK(0);
 
         // ---- phase A: in-window corners become entries, the others red ----
 #pragma unroll 1
@@ -265,6 +272,10 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
             }
 
             // ---- direct reds: the group walks the taps of its pair that have a corner to red ----
+            if (!primary_done) {       // the tap kernel, and so grad_value's zero-fill, are complete and visible
+                pdl_wait_primary();
+                primary_done = true;
+            }
             const size_t slab_off = ((size_t)b * S * M + m) * D + (size_t)sub * VEC;
             float *gbase = grad_value + slab_off;
 #pragma unroll
@@ -297,7 +308,7 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
         const int nwin = tl.nwin;
         if (nwin > 0) {
             __syncthreads();
-            MSDA_REGION_CLOCK(2);
+            MSDA_REGION_CLOCK(1);
             const int n = min(tl.nq, kRegionSlots) * LP_MAX * 4;
             // ---- phase B: counting sort of the entries by window row (phase A counted them) ----
             {   // exclusive scan of cnt[0, nwin): 4 rows per thread
@@ -323,14 +334,10 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
             __syncthreads();
             for (int e = threadIdx.x; e < n; e += kTiledThreads) {
                 const unsigned short r = e_row[e];
-                if (r != kNoRow) {
-                    const int pos = atomicAdd(&cnt[r], 1);
-                    s_coef[pos] = e_coef[e];
-                    s_slot[pos] = (unsigned char)(e / (LP_MAX * 4));
-                }
+                if (r != kNoRow) s_idx[atomicAdd(&cnt[r], 1)] = (unsigned short)e;
             }
-            __syncthreads();          // bucket r is now [r ? cnt[r - 1] : 0, cnt[r]) of s_coef / s_slot
-            MSDA_REGION_CLOCK(3);
+            __syncthreads();          // bucket r is now [r ? cnt[r - 1] : 0, cnt[r]) of s_idx
+            MSDA_REGION_CLOCK(2);
 
             // ---- phase C: one group per touched row, one red per lane ----
             const int b = tl.b, m = tl.m;
@@ -340,8 +347,9 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 4
                 for (int i = beg; i < end; ++i) {
-                    const float cf = s_coef[i];
-                    const float4 gs = gstash[s_slot[i] * LPR + sub];
+                    const int e = s_idx[i];
+                    const float cf = e_coef[e];
+                    const float4 gs = gstash[(e / (LP_MAX * 4)) * LPR + sub];
                     acc.x = fmaf(cf, gs.x, acc.x); acc.y = fmaf(cf, gs.y, acc.y);
                     acc.z = fmaf(cf, gs.z, acc.z); acc.w = fmaf(cf, gs.w, acc.w);
                 }
@@ -354,38 +362,36 @@ region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__rest
             }
         }
         __syncthreads();              // the next tile rewrites tl, the entry list, the stash and the counts
-        MSDA_REGION_CLOCK(nwin > 0 ? 4 : 2);
+        MSDA_REGION_CLOCK(nwin > 0 ? 3 : 1);
     }
 }
 
-// tma: the tap pass stages (x, y, a) with TMA (use_tma_staging on the host: L*P % 4 == 0).
+// The tap pass: grad_loc / grad_attn.  tma: it stages (x, y, a) with TMA (use_tma_staging on the host: L*P % 4 == 0).
 template <int R, int HALO>
-__global__ void __launch_bounds__(kTiledThreads, kRegionMinCtas)
+__global__ void __launch_bounds__(kTiledThreads, kRegionTapCtas)
 msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ value,
                 const int64_t *__restrict__ shapes, const int64_t *__restrict__ lsi,
                 const float *__restrict__ loc, const float *__restrict__ attn,
                 int N, int S, int M, int L, int Lq, int P, unsigned npairs, int tma,
-                float *__restrict__ grad_value, float *__restrict__ grad_loc, float *__restrict__ grad_attn)
+                float *__restrict__ grad_loc, float *__restrict__ grad_attn)
 {
     __shared__ WorkMap wm;
     __shared__ __align__(16) unsigned char slab_mem[kTiledWarps * TapSlab<8>::kBytes];
     __shared__ __align__(8) unsigned long long stage_bar[kTiledWarps * 2];
-    extern __shared__ __align__(128) unsigned char region_dyn[];       // the stage buffers overlay the entry arrays
+    extern __shared__ __align__(128) unsigned char stage_mem[];        // region_tap_smem_bytes()
 
-    MSDA_REGION_CLOCK_INIT;
-    // ---- tap pass: grad_loc / grad_attn (writes nothing the zero-fill writes, so it overlaps the fill) ----
+    pdl_launch_dependents();     // the grad_value kernel's prologue may run on SM slots this kernel frees
     if (tma)
         bwd_tiled_body<float, 4, 32, 16, true, false, false, true, false>(
-            wm, slab_mem, region_dyn, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
+            wm, slab_mem, stage_mem, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
             nullptr, grad_loc, grad_attn, nullptr, 0);
     else
         bwd_tiled_body<float, 4, 32, 16, false, false, false, true, false>(
-            wm, slab_mem, region_dyn, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
+            wm, slab_mem, stage_mem, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
             nullptr, grad_loc, grad_attn, nullptr, 0);
-    __syncthreads();         // the stage buffers are free again
-    MSDA_REGION_CLOCK(0);
-    pdl_wait_primary();      // grad_value's zero-fill (msda_zero_fill as PDL primary) is complete and visible from here on
-    region_grad_value_pass<R, HALO>(grad_out, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, grad_value);
+    // Nothing here writes what the zero-fill writes, but the grad_value kernel relies on this kernel's completion
+    // implying the fill's: wait for the PDL primary last.
+    pdl_wait_primary();
 }
 
 }  // namespace msda
