@@ -32,7 +32,6 @@ def user_problem(cfg, head, seed=0, box_layers=1):
     other branch in fp64 than in fp32 and changes that row's gradient by O(1) -- a property of the MLP, not of the path
     under test (the three-layer MLP is compared with the reference's results on the test pyramid)."""
     c = CONFIGS[cfg]
-    g = torch.Generator().manual_seed(seed)
     masks = []
     for b in range(2):
         lv = []
@@ -43,6 +42,13 @@ def user_problem(cfg, head, seed=0, box_layers=1):
                 m[:, math.ceil(0.75 * w):] = True
             lv.append(m.flatten())
         masks.append(torch.cat(lv))
+    return make_problem(c.shapes, torch.stack(masks), head, seed, box_layers)
+
+
+def make_problem(shapes, mask, head, seed=0, box_layers=1):
+    """user_problem's modules and inputs at any pyramid: mask [N, S] bool; -> (shapes, mods, x)."""
+    n, s = mask.shape
+    g = torch.Generator().manual_seed(seed)
     torch.manual_seed(seed)
     mods = {"enc_output": torch.nn.Linear(256, 256), "enc_output_norm": torch.nn.LayerNorm(256),
             "class_embed": Still_Classifier(256) if head == "still" else VL_Align(256, 768, 0.0, clamp_dot_product=True),
@@ -52,9 +58,9 @@ def user_problem(cfg, head, seed=0, box_layers=1):
         mods["enc_output_norm"].bias.normal_(0.0, 0.1)
     for m in mods.values():
         m.to(DEV)
-    x = {"memory": torch.randn(2, c.S, 256, generator=g).to(DEV), "mask": torch.stack(masks).to(DEV),
-         "lang_feat_pool": torch.randn(2, 768, generator=g).to(DEV)}
-    return c.shapes, mods, x
+    x = {"memory": torch.randn(n, s, 256, generator=g).to(DEV), "mask": mask.to(DEV),
+         "lang_feat_pool": torch.randn(n, 768, generator=g).to(DEV)}
+    return shapes, mods, x
 
 
 def run_fused(shapes, mods, x, k, cot=None):
@@ -94,8 +100,14 @@ def rel(a, b):
                                         ("cfg2", "S", "vl")])
 def test_user_sizes_against_fp64(cfg, k, head):
     shapes, mods, x = user_problem(cfg, head)
+    s = x["memory"].shape[1]
+    check_against_fp64(shapes, mods, x, s if k == "S" else k)
+
+
+def check_against_fp64(shapes, mods, x, k):
+    """Run the kernels forward and backward on random cotangents and assert they match restated_fp64: values and
+    gradients within 2e-4 of scale, the fp64 stable order, the top-k set.  -> (outputs, memory grad, grads, cot)."""
     n, s = x["memory"].shape[:2]
-    k = s if k == "S" else k
     g = torch.Generator().manual_seed(7)
     cot = {"g_class": torch.randn(n, s, 1, generator=g).to(DEV), "g_coord": torch.randn(n, s, 4, generator=g).to(DEV),
            "g_ref": torch.randn(n, k, 4, generator=g).to(DEV)}
@@ -120,6 +132,7 @@ def test_user_sizes_against_fp64(cfg, k, head):
         assert torch.equal(idx[b][clear], order[b, :k][clear]), b
         if k < s:                               # the selected set is the top k
             assert w_cls[b, idx[b], 0].min() >= w_cls[b, order[b, k:], 0].max() - thr
+    return (cls, coord, ref, idx), g_mem, grads, cot
 
 
 def test_exact_ties_invalid_rows_and_nan():

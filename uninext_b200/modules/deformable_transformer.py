@@ -89,7 +89,11 @@ def get_sine_pos_embed(pos_tensor: torch.Tensor, num_pos_feats: int = 128, tempe
                        exchange_xy: bool = True) -> torch.Tensor:
     """[.., Q, n] positions in [0, 1] -> [.., Q, n * num_pos_feats] sine embedding (deformable_transformer_dino.py:612-646):
     component k, feature j = sin / cos (j even / odd) of ``pos_k * 2*pi / temperature ** (2 * (j // 2) / num_pos_feats)``;
-    with ``exchange_xy`` the y block comes first.  CUDA tensors: one hand-written kernel per direction."""
+    with ``exchange_xy`` the y block comes first.  CUDA tensors: one hand-written kernel per direction.  An odd
+    ``num_pos_feats`` raises ValueError: the reference interleaves equal halves of sines and cosines, so it has no
+    value to give."""
+    if num_pos_feats % 2:
+        raise ValueError(f"get_sine_pos_embed takes an even num_pos_feats, got {num_pos_feats}")
     if pos_tensor.is_cuda and pos_tensor.dtype == torch.float32:
         return _SinePosEmbed.apply(pos_tensor, int(num_pos_feats), temperature, bool(exchange_xy))
     dim_t = torch.arange(num_pos_feats, dtype=torch.float32, device=pos_tensor.device)

@@ -111,14 +111,14 @@ class _FlattenLevels(torch.autograd.Function):
             c, level_embed.data_ptr(), src_flat.data_ptr(), pos_flat.data_ptr(), mask_flat.data_ptr(),
             torch.cuda.current_stream().cuda_stream), "msda_flatten_levels_forward_f32")
         ctx.mark_non_differentiable(mask_flat)
-        ctx.cfg = (shapes, n, c)
+        ctx.cfg = (shapes, n, c, level_embed.shape[0])
         return src_flat, pos_flat, mask_flat
 
     @staticmethod
     def backward(ctx, g_src, g_pos, _g_mask):
         from uninext_b200 import _cabi
         lib = _cabi.flatten()
-        shapes, n, c = ctx.cfg
+        shapes, n, c, le_rows = ctx.cfg
         nl = len(shapes)
         need = ctx.needs_input_grad
         want_le, want_src, want_pos = need[0], any(need[2:2 + nl]), any(need[2 + nl:2 + 2 * nl])
@@ -132,7 +132,8 @@ class _FlattenLevels(torch.autograd.Function):
         hs, ws = _ints([h for h, _ in shapes]), _ints([w for _, w in shapes])
         g_le, work, nbytes = None, None, ctypes.c_int64(0)
         if want_le:
-            g_le = torch.empty((nl, c), dtype=torch.float32, device=dev)
+            g_le = torch.empty((le_rows, c), dtype=torch.float32, device=dev)     # rows past L embed no level
+            g_le[nl:].zero_()
             _cabi.check(lib.msda_flatten_levels_workspace(hs, ws, nl, n, c, ctypes.byref(nbytes)),
                         "msda_flatten_levels_workspace")
             work = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
