@@ -45,9 +45,9 @@ def test_header_ctypes_table_and_exports_agree(lib):
     assert lib.msda_abi_version() == 11
 
 
-def test_library_without_the_entry_points_raises(tmp_path):
-    """A library that exports msda_b200.h but not msda_flatten.h loads for the rest of the package, and the
-    input-preparation API raises MSDALibraryError."""
+def test_library_without_the_entry_points_records_them_as_missing(tmp_path):
+    """A library that exports msda_b200.h but not msda_flatten.h loads for the rest of the package, load() records its
+    entry points as missing, and asking for them raises MSDALibraryError."""
     from uninext_b200 import _cabi
     src = tmp_path / "stub.c"
     body = ["int msda_abi_version(void) { return %d; }" % _cabi.ABI_VERSION]
@@ -59,9 +59,12 @@ def test_library_without_the_entry_points_raises(tmp_path):
     except (OSError, subprocess.CalledProcessError) as exc:
         pytest.skip(f"no C compiler: {exc}")
     stub = _cabi.load(str(so))
-    assert set(stub.flatten_missing) == set(_cabi.FLATTEN_SIGNATURES)
+    assert stub.missing == set(_cabi.TWOSTAGE_SIGNATURES) | set(_cabi.FLATTEN_SIGNATURES)
     with pytest.raises(_cabi.MSDALibraryError, match="msda_flatten_"):
         _cabi.flatten(str(so))
+    for name in _cabi.FLATTEN_SIGNATURES:
+        with pytest.raises(_cabi.MSDALibraryError, match=name):
+            _cabi.entry(name, str(so))
 
 
 # ---- argument checks (fake addresses: skipped where a GPU would run the kernels on them) -----------------------------

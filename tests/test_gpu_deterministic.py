@@ -139,22 +139,17 @@ def test_loc_attn_equal_default_path(case):
 
 # ---- 4. chunking changes no bit ------------------------------------------------------------------------------------
 def _call_det_f32(inp, chunk_queries):
-    lib = _cabi.load()
     v = inp["value"]
     n, s, m, d = v.shape
     dims = (n, s, m, d, inp["spatial_shapes"].shape[0], inp["sampling_locations"].shape[1],
             inp["sampling_locations"].shape[4])
-    nbytes = ctypes.c_int64(0)
-    _cabi.check(lib.msda_backward_det_workspace(4, *dims, chunk_queries, ctypes.byref(nbytes)), "workspace")
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=DEV)
+    nbytes = _cabi.workspace("msda_backward_det_workspace", 4, *dims, chunk_queries)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
     gv = torch.full_like(v, float("nan"))                 # the callee zero-fills
     gl = torch.empty_like(inp["sampling_locations"])
     ga = torch.empty_like(inp["attention_weights"])
-    a = _args(inp)
-    code = lib.msda_backward_det_f32(inp["grad_output"].data_ptr(), *(t.data_ptr() for t in a), *dims, gv.data_ptr(),
-                                     gl.data_ptr(), ga.data_ptr(), ws.data_ptr(), ws.numel(),
-                                     torch.cuda.current_stream().cuda_stream)
-    _cabi.check(code, "msda_backward_det_f32")
+    _cabi.call("msda_backward_det_f32", inp["grad_output"], *_args(inp), *dims, gv, gl, ga, ws, ws.numel(),
+               device=v.device)
     return gv, gl, ga, dims
 
 

@@ -128,13 +128,11 @@ def test_input_forms_dtype_and_empty():
 @pytest.mark.parametrize("outs", [(427, 641), (480, 640)], ids=["scalar", "vector"])
 def test_every_element_is_written(binary, outs):
     x = make_logits(5, 50, 84, seed=5)[:, 0].contiguous()
-    lib = _cabi.load()
     if binary:
         out = torch.full((5, *outs), 0xAB, dtype=torch.uint8, device="cuda")
     else:
         out = torch.full((5, *outs), float("nan"), dtype=torch.float32, device="cuda")
-    _cabi.check(lib.msda_mask_paste_f32(x.data_ptr(), 5, 50, 84, 4, 199, 333, outs[0], outs[1], 0.5, binary,
-                                        out.data_ptr(), torch.cuda.current_stream().cuda_stream), "msda_mask_paste_f32")
+    _cabi.call("msda_mask_paste_f32", x, 5, 50, 84, 4, 199, 333, outs[0], outs[1], 0.5, binary, out, device=x.device)
     if binary:
         assert bool(((out == 0) | (out == 1)).all())
         assert torch.equal(out.bool(), paste_masks(x, (199, 333), outs))

@@ -270,18 +270,16 @@ def test_flatten_abi_writes_every_output_element_and_nothing_else(name, c):
     """Outputs, gradients and the workspace pre-filled with NaN (the mask with 0x5a) inside larger buffers: after the
     calls no NaN is left inside, the values are the reference chain's, and the 128 bytes on each side are untouched."""
     from uninext_b200 import _cabi
-    lib = _cabi.flatten()
     shapes, srcs, masks, pos, le = pyramid_inputs(name, c)
     n, nl, s = srcs[0].shape[0], len(shapes), sum(h * w for h, w in shapes)
     hs, ws = (ctypes.c_int * nl)(*[h for h, _ in shapes]), (ctypes.c_int * nl)(*[w for _, w in shapes])
-    stream = torch.cuda.current_stream().cuda_stream
     nan, G = float("nan"), 32
     sf, sf_in = _guarded(n * s * c, torch.float32, nan, G)
     pf, pf_in = _guarded(n * s * c, torch.float32, nan, G)
     mf, mf_in = _guarded(n * s, torch.uint8, 0x5a, 4 * G)
     m8 = [m.view(torch.uint8) for m in masks]
-    assert lib.msda_flatten_levels_forward_f32(_ptrs(srcs), _ptrs(pos), _ptrs(m8), hs, ws, nl, n, c, le.data_ptr(),
-                                               sf_in.data_ptr(), pf_in.data_ptr(), mf_in.data_ptr(), stream) == 0
+    _cabi.call("msda_flatten_levels_forward_f32", _ptrs(srcs), _ptrs(pos), _ptrs(m8), hs, ws, nl, n, c, le, sf_in,
+               pf_in, mf_in, device=le.device)
     src_flat, mask_flat, pos_flat = reference_chain(srcs, masks, pos, le)[:3]
     assert torch.equal(sf_in.view(n, s, c), src_flat) and torch.equal(pf_in.view(n, s, c), pos_flat)
     assert torch.equal(mf_in.view(n, s), mask_flat.view(torch.uint8))
@@ -294,12 +292,10 @@ def test_flatten_abi_writes_every_output_element_and_nothing_else(name, c):
     gs = [_guarded(n * c * h * w, torch.float32, nan, G) for h, w in shapes]
     gp = [_guarded(n * c * h * w, torch.float32, nan, G) for h, w in shapes]
     ge, ge_in = _guarded(nl * c, torch.float32, nan, G)
-    nbytes = ctypes.c_int64()
-    assert lib.msda_flatten_levels_workspace(hs, ws, nl, n, c, ctypes.byref(nbytes)) == 0
-    work = torch.full((nbytes.value // 4,), nan, device=DEV)
-    assert lib.msda_flatten_levels_backward_f32(g_src.data_ptr(), g_pos.data_ptr(), hs, ws, nl, n, c,
-                                                _ptrs([v for _, v in gs]), _ptrs([v for _, v in gp]), ge_in.data_ptr(),
-                                                work.data_ptr(), nbytes.value, stream) == 0
+    nbytes = _cabi.workspace("msda_flatten_levels_workspace", hs, ws, nl, n, c)
+    work = torch.full((nbytes // 4,), nan, device=DEV)
+    _cabi.call("msda_flatten_levels_backward_f32", g_src, g_pos, hs, ws, nl, n, c, _ptrs([v for _, v in gs]),
+               _ptrs([v for _, v in gp]), ge_in, work, nbytes, device=g_src.device)
     st = starts_of(shapes)
     for lvl, (h, w) in enumerate(shapes):
         for g_flat, (buf, inner) in ((g_src, gs[lvl]), (g_pos, gp[lvl])):

@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes
 import os
 
+import torch
+
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "lib", "libmsda_b200.so")
 
@@ -68,8 +70,9 @@ SIGNATURES = {
 }
 ABI_VERSION = 11
 
-# The two-stage query selection's entry points (include/msda_twostage.h), typed by load() when the library exports them;
-# twostage() raises MSDALibraryError for a library that does not.
+# Optional groups: typed by load() when the library exports them; asking for one of a library that does not raises
+# MSDALibraryError (entry(), or twostage() / flatten() for a whole group).  The two-stage query selection
+# (include/msda_twostage.h):
 _i64 = ctypes.c_int64
 TWOSTAGE_SIGNATURES = {
     "msda_twostage_head_forward_f32": (_i, [_vp] * 7 + [_i] * 3 + [ctypes.c_float, _i] + [_vp] * 4 + [_vp]),
@@ -79,7 +82,7 @@ TWOSTAGE_SIGNATURES = {
     "msda_twostage_select_forward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp] * 3 + [_vp, _i64, _vp]),
     "msda_twostage_select_backward_f32": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp]),
 }
-# The encoder's input preparation (include/msda_flatten.h), loaded the same way; flatten() raises for a library without.
+# The encoder's input preparation (include/msda_flatten.h):
 FLATTEN_SIGNATURES = {
     "msda_flatten_levels_forward_f32": (_i, [_vp] * 5 + [_i] * 3 + [_vp] * 4 + [_vp]),
     "msda_flatten_levels_workspace": (_i, [_vp] * 2 + [_i] * 3 + [_vp]),
@@ -115,12 +118,13 @@ def load(path: str | None = None):
         except AttributeError as exc:
             raise MSDALibraryError(f"{p} does not export `{name}` (stale build? run uninext_b200.build --force)") from exc
         fn.restype, fn.argtypes = res, args
-    lib.twostage_missing = [name for name in TWOSTAGE_SIGNATURES if not hasattr(lib, name)]
-    lib.flatten_missing = [name for name in FLATTEN_SIGNATURES if not hasattr(lib, name)]
-    for name, (res, args) in list(TWOSTAGE_SIGNATURES.items()) + list(FLATTEN_SIGNATURES.items()):
+    lib.missing = set()                    # the optional entry points this library does not export
+    for name, (res, args) in {**TWOSTAGE_SIGNATURES, **FLATTEN_SIGNATURES}.items():
         if hasattr(lib, name):
             fn = getattr(lib, name)
             fn.restype, fn.argtypes = res, args
+        else:
+            lib.missing.add(name)
     if lib.msda_abi_version() != ABI_VERSION:
         raise MSDALibraryError(f"{p}: ABI version {lib.msda_abi_version()} != expected {ABI_VERSION}")
     if path is None:
@@ -128,22 +132,58 @@ def load(path: str | None = None):
     return lib
 
 
+_entries = {}
+
+
+def entry(name: str, path: str | None = None):
+    """The typed entry point ``name`` of ``load(path)``.  MSDALibraryError when the library does not export it: an
+    optional group it was built without."""
+    fn = _entries.get(name) if path is None else None
+    if fn is None:
+        lib = load(path)
+        if name in lib.missing:
+            raise MSDALibraryError(f"{path or LIB_PATH} does not export `{name}` (stale build? run "
+                                   "uninext_b200.build --force)")
+        fn = getattr(lib, name)
+        if path is None:
+            _entries[name] = fn
+    return fn
+
+
+def _with_group(table, path):
+    for name in table:
+        entry(name, path)
+    return load(path)
+
+
 def twostage(path: str | None = None):
-    """The loaded library, after checking that it exports the two-stage selection (include/msda_twostage.h)."""
-    lib = load(path)
-    if lib.twostage_missing:
-        raise MSDALibraryError(f"{path or LIB_PATH} does not export `{lib.twostage_missing[0]}` (stale build? run "
-                               "uninext_b200.build --force)")
-    return lib
+    """The library, after checking that it exports the two-stage selection (include/msda_twostage.h)."""
+    return _with_group(TWOSTAGE_SIGNATURES, path)
 
 
 def flatten(path: str | None = None):
-    """The loaded library, after checking that it exports the input preparation (include/msda_flatten.h)."""
-    lib = load(path)
-    if lib.flatten_missing:
-        raise MSDALibraryError(f"{path or LIB_PATH} does not export `{lib.flatten_missing[0]}` (stale build? run "
-                               "uninext_b200.build --force)")
-    return lib
+    """The library, after checking that it exports the input preparation (include/msda_flatten.h)."""
+    return _with_group(FLATTEN_SIGNATURES, path)
+
+
+def call(name: str, *args, device) -> None:
+    """Run entry point ``name`` on ``device``: a tensor argument goes as its ``data_ptr()``, None as NULL, anything else
+    (ints, floats, ctypes objects) unchanged, and the device's current stream is appended as the last argument.  A
+    non-zero return code raises RuntimeError (``check``).  Nothing here synchronises or allocates, so calls can be
+    captured into a CUDA graph."""
+    fn = entry(name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(device):
+        code = fn(*args, torch.cuda.current_stream(device).cuda_stream)
+    if code:
+        check(code, name)
+
+
+def workspace(name: str, *args) -> int:
+    """The size that the query ``name`` writes through its last parameter, an ``int64_t *``."""
+    n = ctypes.c_int64(0)
+    check(entry(name)(*args, ctypes.byref(n)), name)
+    return n.value
 
 
 def check(code: int, what: str) -> None:

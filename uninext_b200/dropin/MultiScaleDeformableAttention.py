@@ -13,8 +13,6 @@ and under ``torch.use_deterministic_algorithms(True)`` the backward sums grad_va
 """
 from __future__ import annotations
 
-import ctypes
-
 import torch
 
 from uninext_b200 import _cabi
@@ -100,29 +98,19 @@ def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_lo
     n, s, m, d, l, lq, p = dims = _dims(value, spatial_shapes, sampling_loc)
     if min(dims) == 0:        # nothing to sample: the reference returns its at::zeros output (cu:54) after a failed empty launch
         return torch.zeros((n, lq, m * d), dtype=value.dtype, device=value.device)
-    lib = _cabi.load()
-    with torch.cuda.device(value.device):
-        out = torch.empty((n, lq, m * d), dtype=value.dtype, device=value.device)
-        stream = torch.cuda.current_stream().cuda_stream
-        fn = getattr(lib, "msda_forward_" + _SUFFIX[value.dtype])
-        code = fn(value.data_ptr(), spatial_shapes.data_ptr(), level_start_index.data_ptr(), sampling_loc.data_ptr(),
-                  attn_weight.data_ptr(), *dims, out.data_ptr(), stream)
-    _cabi.check(code, "ms_deform_attn_forward")
+    out = torch.empty((n, lq, m * d), dtype=value.dtype, device=value.device)
+    _cabi.call("msda_forward_" + _SUFFIX[value.dtype], value, spatial_shapes, level_start_index, sampling_loc,
+               attn_weight, *dims, out, device=value.device)
     return out
 
 
 def _det_workspace(lib, value, dims):
     """Workspace of msda_backward_det_*: the whole call in one pass when it fits DET_WORKSPACE_CAP, otherwise the cap
-    (the library then runs the largest query chunks that fit), and at least one query's worth."""
-    lq = dims[5]
-    need, one = ctypes.c_int64(0), ctypes.c_int64(0)
-    _cabi.check(lib.msda_backward_det_workspace(value.element_size(), *dims, lq, ctypes.byref(need)),
-                "msda_backward_det_workspace")
-    nbytes = need.value
+    (the library then runs the largest query chunks that fit), and at least one query's worth.  ``lib`` is not read
+    (the sizes come from ``_cabi.workspace``); tests and tools call this helper with the loaded library."""
+    nbytes = _cabi.workspace("msda_backward_det_workspace", value.element_size(), *dims, dims[5])
     if nbytes > DET_WORKSPACE_CAP:
-        _cabi.check(lib.msda_backward_det_workspace(value.element_size(), *dims, 1, ctypes.byref(one)),
-                    "msda_backward_det_workspace")
-        nbytes = max(DET_WORKSPACE_CAP, one.value)
+        nbytes = max(DET_WORKSPACE_CAP, _cabi.workspace("msda_backward_det_workspace", value.element_size(), *dims, 1))
     return torch.empty(nbytes, dtype=torch.uint8, device=value.device)
 
 
@@ -146,26 +134,20 @@ def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_l
         gv_dtype = torch.float32 if (value.dtype == torch.bfloat16 and grad_value_dtype == torch.float32) else value.dtype
         return [torch.zeros(value.shape, dtype=gv_dtype, device=value.device), torch.zeros_like(sampling_loc),
                 torch.zeros_like(attn_weight)]
-    lib = _cabi.load()
     det = deterministic_requested() if deterministic is None else bool(deterministic)
-    with torch.cuda.device(value.device):
-        grad_loc = torch.empty_like(sampling_loc)
-        grad_attn = torch.empty_like(attn_weight)
-        stream = torch.cuda.current_stream().cuda_stream
-        common = (grad_output.data_ptr(), value.data_ptr(), spatial_shapes.data_ptr(), level_start_index.data_ptr(),
-                  sampling_loc.data_ptr(), attn_weight.data_ptr(), *dims)
-        ws = _det_workspace(lib, value, dims) if det else None
-        tail = (ws.data_ptr(), ws.numel(), stream) if det else (stream,)
-        kind = "msda_backward_det_" if det else "msda_backward_"
-        if value.dtype == torch.bfloat16:
-            acc = torch.empty(value.shape, dtype=torch.float32, device=value.device)
-            keep_f32 = grad_value_dtype == torch.float32
-            grad_value = acc if keep_f32 else torch.empty_like(value)
-            code = getattr(lib, kind + "bf16")(*common, acc.data_ptr(), None if keep_f32 else grad_value.data_ptr(),
-                                               grad_loc.data_ptr(), grad_attn.data_ptr(), *tail)
-        else:
-            grad_value = torch.empty_like(value)          # zero-filled by the callee on `stream`
-            fn = getattr(lib, kind + _SUFFIX[value.dtype])
-            code = fn(*common, grad_value.data_ptr(), grad_loc.data_ptr(), grad_attn.data_ptr(), *tail)
-    _cabi.check(code, "ms_deform_attn_backward")
+    grad_loc = torch.empty_like(sampling_loc)
+    grad_attn = torch.empty_like(attn_weight)
+    common = (grad_output, value, spatial_shapes, level_start_index, sampling_loc, attn_weight, *dims)
+    ws = _det_workspace(None, value, dims) if det else None
+    tail = (ws, ws.numel()) if det else ()
+    kind = "msda_backward_det_" if det else "msda_backward_"
+    if value.dtype == torch.bfloat16:
+        acc = torch.empty(value.shape, dtype=torch.float32, device=value.device)
+        keep_f32 = grad_value_dtype == torch.float32
+        grad_value = acc if keep_f32 else torch.empty_like(value)
+        _cabi.call(kind + "bf16", *common, acc, None if keep_f32 else grad_value, grad_loc, grad_attn, *tail,
+                   device=value.device)
+    else:
+        grad_value = torch.empty_like(value)          # zero-filled by the callee on the current stream
+        _cabi.call(kind + _SUFFIX[value.dtype], *common, grad_value, grad_loc, grad_attn, *tail, device=value.device)
     return [grad_value, grad_loc, grad_attn]

@@ -25,10 +25,6 @@ from uninext_b200._determinism import deterministic_requested
 from uninext_b200._precision import tf32_allowed
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def _f32c(t):
     return t.contiguous() if t.dtype == torch.float32 else t.float().contiguous()
 
@@ -46,8 +42,7 @@ def colsum(x2d: torch.Tensor) -> torch.Tensor:
     if cols % 4 or x2d.data_ptr() % 16 or deterministic_requested():
         return x2d.sum(0)
     out = torch.empty(cols, dtype=torch.float32, device=x2d.device)
-    with torch.cuda.device(x2d.device):
-        _cabi.check(_cabi.load().msda_colsum_f32(x2d.data_ptr(), rows, cols, out.data_ptr(), _stream()), "msda_colsum_f32")
+    _cabi.call("msda_colsum_f32", x2d, rows, cols, out, device=x2d.device)
     return out
 
 
@@ -79,10 +74,7 @@ def tcgen05_linear(x2: torch.Tensor, weight: torch.Tensor, bias) -> torch.Tensor
     m, k = x2.shape
     n = weight.shape[0]
     out = torch.empty((m, n), dtype=torch.float32, device=x2.device)
-    with torch.cuda.device(x2.device):
-        _cabi.check(_cabi.load().msda_linear_tf32(x2.data_ptr(), weight.data_ptr(),
-                                                  bias.data_ptr() if bias is not None else None, m, n, k, out.data_ptr(),
-                                                  _stream()), "msda_linear_tf32")
+    _cabi.call("msda_linear_tf32", x2, weight, bias, m, n, k, out, device=x2.device)
     return out
 
 
@@ -119,10 +111,7 @@ def tcgen05_linear_ex(x2, weight, bias, row_mask=None, relu=False):
     if row_mask is not None:
         mask8 = row_mask.reshape(-1).contiguous()
         mask8 = mask8.view(torch.uint8) if mask8.dtype == torch.bool else mask8.to(torch.uint8)       # bool is one byte: no copy
-    with torch.cuda.device(x2.device):
-        _cabi.check(_cabi.load().msda_linear_tf32_ex(x2.data_ptr(), weight.data_ptr(), bias.data_ptr() if bias is not None else None,
-                                                     mask8.data_ptr() if mask8 is not None else None, m, n, k, int(relu),
-                                                     out.data_ptr(), _stream()), "msda_linear_tf32_ex")
+    _cabi.call("msda_linear_tf32_ex", x2, weight, bias, mask8, m, n, k, int(relu), out, device=x2.device)
     return out
 
 
@@ -169,10 +158,7 @@ class _LinearColsum(Function):
             # ReLU backward and the bias gradient in ONE pass over (g, y)  (masked rows have y == 0: zeroed by the same test)
             out = torch.empty_like(g2)
             gb = torch.empty(g2.shape[1], dtype=torch.float32, device=g2.device)
-            with torch.cuda.device(g2.device):
-                _cabi.check(_cabi.load().msda_relu_backward_colsum_f32(g2.data_ptr(), y.data_ptr(), g2.shape[0], g2.shape[1],
-                                                                       out.data_ptr(), gb.data_ptr(), _stream()),
-                            "msda_relu_backward_colsum_f32")
+            _cabi.call("msda_relu_backward_colsum_f32", g2, y, g2.shape[0], g2.shape[1], out, gb, device=g2.device)
             g2 = out
         elif ctx.relu:
             g2 = torch.ops.aten.threshold_backward(g2, y, 0.0)          # masked rows have y == 0: already zeroed
@@ -240,7 +226,6 @@ class _SamplingPrologue(Function):
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)      # like the reference module (ms_deform_attn.py:78)
     def forward(ctx, query, w_off, b_off, w_attn, b_attn, ref, shapes, n_heads, n_levels, n_points, gemm):
-        lib = _cabi.load()
         q2 = query.reshape(-1, query.shape[-1])
         rows = q2.shape[0]
         weight = torch.cat((w_off, w_attn), 0)                    # [M*LP*3, C]: offsets first, logits last
@@ -249,10 +234,8 @@ class _SamplingPrologue(Function):
         ref_c = _f32c(ref).reshape(rows, n_levels, ref.shape[-1])
         loc = torch.empty((rows, n_heads, n_levels, n_points, 2), dtype=torch.float32, device=query.device)
         attn = torch.empty((rows, n_heads, n_levels, n_points), dtype=torch.float32, device=query.device)
-        with torch.cuda.device(query.device):
-            _cabi.check(lib.msda_prologue_forward_f32(proj.data_ptr(), ref_c.data_ptr(), shapes.data_ptr(), rows, n_heads,
-                                                      n_levels, n_points, ref.shape[-1], loc.data_ptr(), attn.data_ptr(),
-                                                      _stream()), "msda_prologue_forward_f32")
+        _cabi.call("msda_prologue_forward_f32", proj, ref_c, shapes, rows, n_heads, n_levels, n_points, ref.shape[-1],
+                   loc, attn, device=query.device)
         ctx.save_for_backward(q2, weight, attn, ref_c, shapes)
         ctx.dims = (n_heads, n_levels, n_points, ref.shape[-1], w_off.shape[0], query.shape)
         lead = query.shape[:-1]
@@ -262,16 +245,13 @@ class _SamplingPrologue(Function):
     @once_differentiable
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, g_loc, g_attn):
-        lib = _cabi.load()
         q2, weight, attn, ref_c, shapes = ctx.saved_tensors
         m, l, p, rd, n_off, qshape = ctx.dims
         rows = q2.shape[0]
         g_proj = torch.empty((rows, weight.shape[0]), dtype=torch.float32, device=q2.device)
         g_loc, g_attn = _aligned(_f32c(g_loc), 8), _f32c(g_attn)             # grad_loc is read as float2
-        with torch.cuda.device(q2.device):
-            _cabi.check(lib.msda_prologue_backward_f32(g_loc.data_ptr(), g_attn.data_ptr(), attn.data_ptr(), ref_c.data_ptr(),
-                                                       shapes.data_ptr(), rows, m, l, p, rd, g_proj.data_ptr(), _stream()),
-                        "msda_prologue_backward_f32")
+        _cabi.call("msda_prologue_backward_f32", g_loc, g_attn, attn, ref_c, shapes, rows, m, l, p, rd, g_proj,
+                   device=q2.device)
         gq = torch.mm(g_proj, weight).view(qshape) if ctx.needs_input_grad[0] else None
         gw = weight_grad(g_proj, q2)
         gb = colsum(g_proj)
@@ -290,7 +270,6 @@ class _AddLayerNorm(Function):
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)      # autocast runs layer_norm in fp32 too
     def forward(ctx, a, b, gamma, beta, eps):
-        lib = _cabi.load()
         cols = a.shape[-1]
         a2 = a.reshape(-1, cols).contiguous()
         b2 = b.reshape(-1, cols).contiguous() if b is not None else None
@@ -299,12 +278,8 @@ class _AddLayerNorm(Function):
         z = torch.empty_like(a2) if b2 is not None else a2
         mean = torch.empty(rows, dtype=torch.float32, device=a.device)
         rstd = torch.empty(rows, dtype=torch.float32, device=a.device)
-        with torch.cuda.device(a.device):
-            _cabi.check(lib.msda_add_layernorm_forward_f32(a2.data_ptr(), b2.data_ptr() if b2 is not None else None,
-                                                           gamma.data_ptr(), beta.data_ptr(), rows, cols, float(eps),
-                                                           z.data_ptr() if b2 is not None else None, y.data_ptr(),
-                                                           mean.data_ptr(), rstd.data_ptr(), _stream()),
-                        "msda_add_layernorm_forward_f32")
+        _cabi.call("msda_add_layernorm_forward_f32", a2, b2, gamma, beta, rows, cols, float(eps),
+                   z if b2 is not None else None, y, mean, rstd, device=a.device)
         ctx.save_for_backward(z, gamma, mean, rstd)
         ctx.has_b = b is not None
         ctx.a_dtype, ctx.b_dtype = a.dtype, (b.dtype if b is not None else None)
@@ -314,17 +289,14 @@ class _AddLayerNorm(Function):
     @once_differentiable
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, gy):
-        lib = _cabi.load()
         z, gamma, mean, rstd = ctx.saved_tensors
         rows, cols = z.shape
         gy2 = _aligned(_f32c(gy.reshape(rows, cols)))
         dz = torch.empty_like(z)
         dgamma = torch.empty_like(gamma)
         dbeta = torch.empty_like(gamma)
-        with torch.cuda.device(z.device):
-            _cabi.check(lib.msda_layernorm_backward_f32(gy2.data_ptr(), z.data_ptr(), gamma.data_ptr(), mean.data_ptr(),
-                                                        rstd.data_ptr(), rows, cols, dz.data_ptr(), dgamma.data_ptr(),
-                                                        dbeta.data_ptr(), _stream()), "msda_layernorm_backward_f32")
+        _cabi.call("msda_layernorm_backward_f32", gy2, z, gamma, mean, rstd, rows, cols, dz, dgamma, dbeta,
+                   device=z.device)
         dz = dz.view(gy.shape)
         da = dz.to(ctx.a_dtype) if ctx.a_dtype != dz.dtype else dz
         db = (dz.to(ctx.b_dtype) if ctx.b_dtype != dz.dtype else dz) if ctx.has_b else None

@@ -15,6 +15,8 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from uninext_b200 import _cabi
+
 from .deformable_layers import DeformableTransformerDecoderLayer, fp32_under_autocast
 from .ms_deform_attn import batched_value_proj, use_batched_value_proj
 
@@ -56,32 +58,23 @@ class _SinePosEmbed(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pos, num_pos_feats, temperature, exchange_xy):
-        from uninext_b200 import _cabi
-        lib = _cabi.load()
         p2 = pos.contiguous().float()
         n = p2.shape[-1]
         r = p2.numel() // n
         out = torch.empty((*p2.shape[:-1], n * num_pos_feats), dtype=torch.float32, device=pos.device)
-        with torch.cuda.device(pos.device):
-            _cabi.check(lib.msda_sine_pos_embed_forward_f32(p2.data_ptr(), r, n, num_pos_feats, float(temperature), int(exchange_xy),
-                                                            out.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                        "msda_sine_pos_embed_forward_f32")
+        _cabi.call("msda_sine_pos_embed_forward_f32", p2, r, n, num_pos_feats, float(temperature), int(exchange_xy),
+                   out, device=pos.device)
         ctx.save_for_backward(p2)
         ctx.cfg = (r, n, num_pos_feats, float(temperature), int(exchange_xy), pos.dtype)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        from uninext_b200 import _cabi
-        lib = _cabi.load()
         (p2,) = ctx.saved_tensors
         r, n, f, t, xy, dt = ctx.cfg
         g = g.contiguous().float()
         gp = torch.empty_like(p2)
-        with torch.cuda.device(p2.device):
-            _cabi.check(lib.msda_sine_pos_embed_backward_f32(p2.data_ptr(), g.data_ptr(), r, n, f, t, xy, gp.data_ptr(),
-                                                             torch.cuda.current_stream().cuda_stream),
-                        "msda_sine_pos_embed_backward_f32")
+        _cabi.call("msda_sine_pos_embed_backward_f32", p2, g, r, n, f, t, xy, gp, device=p2.device)
         return gp.to(dt), None, None, None
 
 
@@ -167,15 +160,11 @@ def get_reference_points(spatial_shapes, valid_ratios, device=None):
     and is cached; per call only one divide and one multiply remain."""
     device = device or valid_ratios.device
     if valid_ratios.is_cuda and valid_ratios.dtype == torch.float32 and not valid_ratios.requires_grad:
-        from uninext_b200 import _cabi
         ss, lsi, s_total = _level_args(spatial_shapes, None, valid_ratios.device)
         n, l = valid_ratios.shape[0], ss.shape[0]
         vr = valid_ratios.contiguous()
         ref = torch.empty((n, s_total, l, 2), dtype=torch.float32, device=vr.device)
-        with torch.cuda.device(vr.device):
-            _cabi.check(_cabi.load().msda_encoder_ref_points_f32(vr.data_ptr(), ss.data_ptr(), lsi.data_ptr(), n, s_total, l,
-                                                                 ref.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                        "msda_encoder_ref_points_f32")
+        _cabi.call("msda_encoder_ref_points_f32", vr, ss, lsi, n, s_total, l, ref, device=vr.device)
         return ref
     xy, wh, lvl = _pixel_centres(_shapes_key(spatial_shapes), device)
     ref = xy[None] / (valid_ratios[:, lvl] * wh[None])                  # [N, S, 2]
@@ -191,21 +180,15 @@ def gen_encoder_output_proposals(memory_padding_mask, spatial_shapes, base_scale
     n = memory_padding_mask.shape[0]
     device = memory_padding_mask.device
     if memory_padding_mask.is_cuda:                 # two launches: valid extents per (image, level), then the proposals
-        from uninext_b200 import _cabi
-        lib = _cabi.load()
         ss, lsi, s_total = _level_args(spatial_shapes, None, device)
         l = ss.shape[0]
         m8 = memory_padding_mask.to(torch.uint8).contiguous()
         counts = torch.empty((n, l, 2), dtype=torch.int32, device=device)
         prop = torch.empty((n, s_total, 4), dtype=torch.float32, device=device)
         keep = torch.empty((n, s_total, 1), dtype=torch.uint8, device=device)
-        with torch.cuda.device(device):
-            st = torch.cuda.current_stream().cuda_stream
-            _cabi.check(lib.msda_valid_counts(m8.data_ptr(), ss.data_ptr(), lsi.data_ptr(), n, s_total, l, counts.data_ptr(), st),
-                        "msda_valid_counts")
-            _cabi.check(lib.msda_encoder_proposals_f32(m8.data_ptr(), counts.data_ptr(), ss.data_ptr(), lsi.data_ptr(), n, s_total,
-                                                       l, float(base_scale), prop.data_ptr(), keep.data_ptr(), st),
-                        "msda_encoder_proposals_f32")
+        _cabi.call("msda_valid_counts", m8, ss, lsi, n, s_total, l, counts, device=device)
+        _cabi.call("msda_encoder_proposals_f32", m8, counts, ss, lsi, n, s_total, l, float(base_scale), prop, keep,
+                   device=device)
         return prop, keep.bool()
     xy, wh, lvl = _pixel_centres(shapes, device)
     counts, cur = [], 0

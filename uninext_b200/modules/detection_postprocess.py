@@ -15,7 +15,6 @@ same outputs without a host round trip, so it can be captured into a CUDA graph 
 """
 from __future__ import annotations
 
-import ctypes
 import functools
 from typing import Dict, NamedTuple, Optional, Sequence, Tuple, Union
 
@@ -134,19 +133,13 @@ def postprocess_detections(box_cls: torch.Tensor, box_pred: torch.Tensor, positi
             _CAPTURED[id(held)] = held
     x = box_cls.float().contiguous()
     bx = box_pred.float().contiguous()
-    lib = _cabi.load()
-    ws_bytes = ctypes.c_int64(0)
-    _cabi.check(lib.msda_detpost_workspace(b, q, t, c, k, ctypes.byref(ws_bytes)), "msda_detpost_workspace")
+    ws_bytes = _cabi.workspace("msda_detpost_workspace", b, q, t, c, k)
     out = Detections(torch.empty((b, k), dtype=torch.float32, device=dev), torch.empty((b, k), dtype=torch.int32, device=dev),
                      torch.empty((b, k, 4), dtype=torch.float32, device=dev),
                      torch.empty((b, k), dtype=torch.int32, device=dev), torch.empty((b,), dtype=torch.int32, device=dev))
-    ws = torch.empty(max(int(ws_bytes.value), 16), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(lib.msda_detpost_f32(x.data_ptr(), bx.data_ptr(), iou_pred.data_ptr() if iou_pred is not None else None,
-                                         class_start.data_ptr(), tokens.data_ptr(), sizes.data_ptr(), b, q, t, c,
-                                         int(nms_iou is not None), float(nms_iou) if nms_iou is not None else 0.0, k,
-                                         out.scores.data_ptr(), out.labels.data_ptr(), out.query_index.data_ptr(),
-                                         out.boxes.data_ptr(), out.count.data_ptr(), ws.data_ptr(), ws.numel(),
-                                         torch.cuda.current_stream().cuda_stream), "msda_detpost_f32")
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=dev)
+    _cabi.call("msda_detpost_f32", x, bx, iou_pred, class_start, tokens, sizes, b, q, t, c, int(nms_iou is not None),
+               float(nms_iou) if nms_iou is not None else 0.0, k, out.scores, out.labels, out.query_index, out.boxes,
+               out.count, ws, ws.numel(), device=dev)
     return out
 

@@ -23,6 +23,8 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from uninext_b200 import _cabi
+
 from .deformable_layers import DeformableTransformerDecoderLayer, DeformableTransformerEncoderLayer
 from .deformable_transformer import (_LEVEL_TENSORS, DeformableTransformerDecoder, _level_args, _shapes_key,
                                      get_reference_points)
@@ -97,8 +99,6 @@ class _FlattenLevels(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, level_embed, shapes, *tensors):
-        from uninext_b200 import _cabi
-        lib = _cabi.flatten()
         nl = len(shapes)
         srcs, pos, masks = tensors[:nl], tensors[nl:2 * nl], tensors[2 * nl:]
         n, c = srcs[0].shape[:2]
@@ -106,18 +106,15 @@ class _FlattenLevels(torch.autograd.Function):
         src_flat = level_embed.new_empty((n, s, c))
         pos_flat = level_embed.new_empty((n, s, c))
         mask_flat = torch.empty((n, s), dtype=torch.uint8, device=level_embed.device)
-        _cabi.check(lib.msda_flatten_levels_forward_f32(
-            _ptrs(srcs), _ptrs(pos), _ptrs(masks), _ints([h for h, _ in shapes]), _ints([w for _, w in shapes]), nl, n,
-            c, level_embed.data_ptr(), src_flat.data_ptr(), pos_flat.data_ptr(), mask_flat.data_ptr(),
-            torch.cuda.current_stream().cuda_stream), "msda_flatten_levels_forward_f32")
+        _cabi.call("msda_flatten_levels_forward_f32", _ptrs(srcs), _ptrs(pos), _ptrs(masks),
+                   _ints([h for h, _ in shapes]), _ints([w for _, w in shapes]), nl, n, c, level_embed, src_flat,
+                   pos_flat, mask_flat, device=level_embed.device)
         ctx.mark_non_differentiable(mask_flat)
         ctx.cfg = (shapes, n, c, level_embed.shape[0])
         return src_flat, pos_flat, mask_flat
 
     @staticmethod
     def backward(ctx, g_src, g_pos, _g_mask):
-        from uninext_b200 import _cabi
-        lib = _cabi.flatten()
         shapes, n, c, le_rows = ctx.cfg
         nl = len(shapes)
         need = ctx.needs_input_grad
@@ -130,18 +127,15 @@ class _FlattenLevels(torch.autograd.Function):
         g_src = (zeros() if g_src is None else g_src.contiguous()) if want_src else None
         g_pos = (zeros() if g_pos is None else g_pos.contiguous()) if (want_pos or want_le) else None
         hs, ws = _ints([h for h, _ in shapes]), _ints([w for _, w in shapes])
-        g_le, work, nbytes = None, None, ctypes.c_int64(0)
+        g_le, work, nbytes = None, None, 0
         if want_le:
             g_le = torch.empty((le_rows, c), dtype=torch.float32, device=dev)     # rows past L embed no level
             g_le[nl:].zero_()
-            _cabi.check(lib.msda_flatten_levels_workspace(hs, ws, nl, n, c, ctypes.byref(nbytes)),
-                        "msda_flatten_levels_workspace")
-            work = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()
-        _cabi.check(lib.msda_flatten_levels_backward_f32(
-            ptr(g_src), ptr(g_pos), hs, ws, nl, n, c, None if grad_src is None else _ptrs(grad_src),
-            None if grad_pos is None else _ptrs(grad_pos), ptr(g_le), ptr(work), nbytes.value,
-            torch.cuda.current_stream().cuda_stream), "msda_flatten_levels_backward_f32")
+            nbytes = _cabi.workspace("msda_flatten_levels_workspace", hs, ws, nl, n, c)
+            work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _cabi.call("msda_flatten_levels_backward_f32", g_src, g_pos, hs, ws, nl, n, c,
+                   None if grad_src is None else _ptrs(grad_src), None if grad_pos is None else _ptrs(grad_pos), g_le,
+                   work, nbytes, device=dev)
         per_level = lambda grads, i: None if grads is None or not need[i] else grads[(i - 2) % nl]
         return (g_le, None, *[per_level(grad_src, 2 + i) for i in range(nl)],
                 *[per_level(grad_pos, 2 + nl + i) for i in range(nl)], *[None] * nl)
@@ -194,19 +188,15 @@ def flatten_levels(srcs, masks, pos_embeds, level_embed):
         return (torch.cat(src_flatten, 1), torch.cat(mask_flatten, 1), torch.cat(lvl_pos_embed_flatten, 1), spatial_shapes,
                 level_start_index, torch.stack(ratios, 1))
     _check_cuda(srcs, masks, pos_embeds, level_embed)
-    from uninext_b200 import _cabi
     dev = level_embed.device
     n, nl = srcs[0].shape[0], len(srcs)
-    with torch.cuda.device(dev):
-        src_flat, pos_flat, mask_flat = _FlattenLevels.apply(
-            level_embed, shapes, *[s.contiguous() for s in srcs], *[p.contiguous() for p in pos_embeds],
-            *[m.contiguous().view(torch.uint8) for m in masks])
-        ss, lsi, s_total = _level_args(shapes, None, dev)
-        counts = torch.empty((n, nl, 2), dtype=torch.int32, device=dev)              # (valid W, valid H)
-        _cabi.check(_cabi.load().msda_valid_counts(mask_flat.data_ptr(), ss.data_ptr(), lsi.data_ptr(), n, s_total, nl,
-                                                   counts.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                    "msda_valid_counts")
-        valid_ratios = counts.float() * _level_inv_sizes(shapes, dev)               # valid.float() / H, as get_valid_ratio
+    src_flat, pos_flat, mask_flat = _FlattenLevels.apply(
+        level_embed, shapes, *[s.contiguous() for s in srcs], *[p.contiguous() for p in pos_embeds],
+        *[m.contiguous().view(torch.uint8) for m in masks])
+    ss, lsi, s_total = _level_args(shapes, None, dev)
+    counts = torch.empty((n, nl, 2), dtype=torch.int32, device=dev)              # (valid W, valid H)
+    _cabi.call("msda_valid_counts", mask_flat, ss, lsi, n, s_total, nl, counts, device=dev)
+    valid_ratios = counts.float() * _level_inv_sizes(shapes, dev)               # valid.float() / H, as get_valid_ratio
     return src_flat, mask_flat.view(torch.bool), pos_flat, ss, lsi, valid_ratios
 
 

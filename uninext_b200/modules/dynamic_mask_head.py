@@ -46,34 +46,24 @@ def dynamic_param_counts(controller_layers: int = 3, rel_coord: bool = True, in_
     return weight_nums, bias_nums
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 class _AlignedBilinear(Function):
     @staticmethod
     def forward(ctx, x, factor):
-        lib = _cabi.load()
         x = x.contiguous().float()
         *lead, h, w = x.shape
         planes = math.prod(lead) if lead else 1
         out = torch.empty((*lead, h * factor, w * factor), dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            _cabi.check(lib.msda_aligned_bilinear_forward_f32(x.data_ptr(), planes, h, w, factor, out.data_ptr(), _stream()),
-                        "msda_aligned_bilinear_forward_f32")
+        _cabi.call("msda_aligned_bilinear_forward_f32", x, planes, h, w, factor, out, device=x.device)
         ctx.dims = (planes, h, w, factor, x.shape)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        lib = _cabi.load()
         planes, h, w, factor, shape = ctx.dims
         g = g.contiguous().float()
         gin = torch.empty(shape, dtype=torch.float32, device=g.device)
-        with torch.cuda.device(g.device):
-            _cabi.check(lib.msda_aligned_bilinear_backward_f32(g.data_ptr(), planes, h, w, factor, gin.data_ptr(), _stream()),
-                        "msda_aligned_bilinear_backward_f32")
+        _cabi.call("msda_aligned_bilinear_backward_f32", g, planes, h, w, factor, gin, device=g.device)
         return gin, None
 
 
@@ -90,15 +80,12 @@ def aligned_bilinear(tensor: torch.Tensor, factor: int) -> torch.Tensor:
 class _DynamicMaskHead(Function):
     @staticmethod
     def forward(ctx, feats, params, refs, inst_start, max_inst, stride, rel_coord):
-        lib = _cabi.load()
         feats, params, refs = feats.contiguous().float(), params.contiguous().float(), refs.contiguous().float()
         n, c, h, w = feats.shape
         i = params.shape[0]
         logits = torch.empty((i, h, w), dtype=torch.float32, device=feats.device)
-        with torch.cuda.device(feats.device):
-            _cabi.check(lib.msda_condinst_forward_f32(feats.data_ptr(), params.data_ptr(), refs.data_ptr(), inst_start.data_ptr(),
-                                                      n, h, w, i, max_inst, stride, int(rel_coord), logits.data_ptr(),
-                                                      _stream()), "msda_condinst_forward_f32")
+        _cabi.call("msda_condinst_forward_f32", feats, params, refs, inst_start, n, h, w, i, max_inst, stride,
+                   int(rel_coord), logits, device=feats.device)
         ctx.save_for_backward(feats, params, refs, inst_start)
         ctx.cfg = (stride, int(rel_coord), int(max_inst))
         return logits
@@ -107,17 +94,14 @@ class _DynamicMaskHead(Function):
     @once_differentiable
     def backward(ctx, g):
         alert_not_deterministic("_DynamicMaskHead.backward (msda_condinst_backward_f32 sums with float atomics)")
-        lib = _cabi.load()
         feats, params, refs, inst_start = ctx.saved_tensors
         stride, rel, max_inst = ctx.cfg
         n, c, h, w = feats.shape
         i = params.shape[0]
         g = g.contiguous().float()
         gf, gp, gr = torch.empty_like(feats), torch.empty_like(params), torch.empty_like(refs)
-        with torch.cuda.device(feats.device):
-            _cabi.check(lib.msda_condinst_backward_f32(g.data_ptr(), feats.data_ptr(), params.data_ptr(), refs.data_ptr(),
-                                                       inst_start.data_ptr(), n, h, w, i, max_inst, stride, rel, gf.data_ptr(),
-                                                       gp.data_ptr(), gr.data_ptr(), _stream()), "msda_condinst_backward_f32")
+        _cabi.call("msda_condinst_backward_f32", g, feats, params, refs, inst_start, n, h, w, i, max_inst, stride, rel,
+                   gf, gp, gr, device=feats.device)
         return gf, gp, gr, None, None, None, None
 
 

@@ -17,7 +17,6 @@ dicts, computed on the device (csrc/msda_maskrle.cuh, DESIGN.md section 3.14) wi
 """
 from __future__ import annotations
 
-import ctypes
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -66,11 +65,8 @@ def paste_masks(mask_logits: torch.Tensor, image_size: Sequence[int], output_siz
     out = torch.empty((i, out_h, out_w), dtype=torch.uint8 if binary else torch.float32, device=mask_logits.device)
     if i > 0:
         x = mask_logits.float().contiguous()
-        lib = _cabi.load()
-        with torch.cuda.device(x.device):
-            _cabi.check(lib.msda_mask_paste_f32(x.data_ptr(), i, hs, ws, stride, h, w, out_h, out_w,
-                                                float(threshold) if binary else 0.0, int(binary), out.data_ptr(),
-                                                torch.cuda.current_stream().cuda_stream), "msda_mask_paste_f32")
+        _cabi.call("msda_mask_paste_f32", x, i, hs, ws, stride, h, w, out_h, out_w, float(threshold) if binary else 0.0,
+                   int(binary), out, device=x.device)
     return out.view(torch.bool) if binary else out
 
 
@@ -112,10 +108,8 @@ def paste_masks_rle(mask_logits: torch.Tensor, image_size: Sequence[int], output
     if i == 0:
         return []
     x = mask_logits.float().contiguous()
-    lib = _cabi.load()
-    return _encode(x.device, i, out_h, out_w, lambda ws_ptr, ws_bytes, stream: (
-        lib.msda_mask_rle_count_f32(x.data_ptr(), i, hs, ws, stride, h, w, out_h, out_w, float(threshold), ws_ptr,
-                                    ws_bytes, stream), "msda_mask_rle_count_f32"))
+    return _encode(x.device, i, out_h, out_w, "msda_mask_rle_count_f32", x, i, hs, ws, stride, h, w, out_h, out_w,
+                   float(threshold))
 
 
 def encode_masks_rle(masks: torch.Tensor) -> List[dict]:
@@ -139,31 +133,25 @@ def encode_masks_rle(masks: torch.Tensor) -> List[dict]:
     m = masks.contiguous()
     if m.dtype == torch.bool:
         m = m.view(torch.uint8)
-    lib = _cabi.load()
-    return _encode(m.device, i, out_h, out_w, lambda ws_ptr, ws_bytes, stream: (
-        lib.msda_mask_rle_count_u8(m.data_ptr(), i, out_h, out_w, ws_ptr, ws_bytes, stream), "msda_mask_rle_count_u8"))
+    return _encode(m.device, i, out_h, out_w, "msda_mask_rle_count_u8", m, i, out_h, out_w)
 
 
-def _encode(device, i, out_h, out_w, count) -> List[dict]:
-    """Both steps of a call.  Two host synchronisations: one reads the number of boundaries B, which sizes the positions
-    (4 B each) and the characters (at most 7 per count, B + I counts); one brings the offsets and characters back."""
-    lib = _cabi.load()
-    n = ctypes.c_int64(0)
-    _cabi.check(lib.msda_mask_rle_workspace(i, out_h, out_w, ctypes.byref(n)), "msda_mask_rle_workspace")
-    with torch.cuda.device(device):
-        stream = torch.cuda.current_stream()
-        ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-        _cabi.check(*count(ws.data_ptr(), n.value, stream.cuda_stream))
-        boundaries = int(ws[: 8 * (i * out_w + 1)].view(torch.int64)[-1])                    # synchronisation 1
-        pos = torch.empty(4 * boundaries, dtype=torch.uint8, device=device)
-        head = 8 * (i + 1)
-        out = torch.empty(head + 7 * (boundaries + i), dtype=torch.uint8, device=device)     # byte offsets, characters
-        _cabi.check(lib.msda_mask_rle_encode(i, out_h, out_w, boundaries, ws.data_ptr(), n.value,
-                                             pos.data_ptr() if boundaries else None, out.data_ptr(),
-                                             out.data_ptr() + head, stream.cuda_stream), "msda_mask_rle_encode")
-        host = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
-        host.copy_(out, non_blocking=True)
-        stream.synchronize()                                                                 # synchronisation 2
+def _encode(device, i, out_h, out_w, count, *count_args) -> List[dict]:
+    """Both steps of a call: the entry point ``count`` on ``count_args`` and the workspace, then msda_mask_rle_encode.
+    Two host synchronisations: one reads the number of boundaries B, which sizes the positions (4 B each) and the
+    characters (at most 7 per count, B + I counts); one brings the offsets and characters back."""
+    n = _cabi.workspace("msda_mask_rle_workspace", i, out_h, out_w)
+    ws = torch.empty(n, dtype=torch.uint8, device=device)
+    _cabi.call(count, *count_args, ws, n, device=device)
+    boundaries = int(ws[: 8 * (i * out_w + 1)].view(torch.int64)[-1])                    # synchronisation 1
+    pos = torch.empty(4 * boundaries, dtype=torch.uint8, device=device)
+    head = 8 * (i + 1)
+    out = torch.empty(head + 7 * (boundaries + i), dtype=torch.uint8, device=device)     # byte offsets, characters
+    _cabi.call("msda_mask_rle_encode", i, out_h, out_w, boundaries, ws, n, pos if boundaries else None, out,
+               out.data_ptr() + head, device=device)
+    host = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
+    host.copy_(out, non_blocking=True)                                                   # on device's current stream
+    torch.cuda.current_stream(device).synchronize()                                      # synchronisation 2
     buf = host.numpy()
     offs = buf[:head].view(np.int64)
     data = buf[head:head + int(offs[i])].tobytes()

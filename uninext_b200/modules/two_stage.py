@@ -12,12 +12,13 @@ CPU tensors run the reference's torch chain.  Any other width or dtype on the GP
 """
 from __future__ import annotations
 
-import ctypes
 import math
 
 import torch
 import torch.nn.functional as F
 from torch import nn
+
+from uninext_b200 import _cabi
 
 from .deformable_transformer import gen_encoder_output_proposals
 
@@ -72,47 +73,33 @@ class VL_Align(nn.Module):
         return u, torch.matmul(e, self.bias_lang) + self.bias0, self.clamp_dot_product
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 class _Head(torch.autograd.Function):
     """y = enc_output(memory) -> (om = LayerNorm(keep ? y : b_e), logit = clamp(om . u[n] + c[n]))."""
 
     @staticmethod
     def forward(ctx, y, keep, b_e, gamma, beta, u, c, clamp, eps):
-        from uninext_b200 import _cabi
-        lib = _cabi.twostage()
         n, s, w = y.shape
         om = torch.empty_like(y)
         logit = y.new_empty((n, s, 1))
         mean, rstd = y.new_empty((n, s)), y.new_empty((n, s))
-        _cabi.check(lib.msda_twostage_head_forward_f32(y.data_ptr(), keep.data_ptr(), b_e.data_ptr(), gamma.data_ptr(),
-                                                       beta.data_ptr(), u.data_ptr(), c.data_ptr(), n, s, w, eps, int(clamp),
-                                                       om.data_ptr(), logit.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
-                                                       _stream()), "msda_twostage_head_forward_f32")
+        _cabi.call("msda_twostage_head_forward_f32", y, keep, b_e, gamma, beta, u, c, n, s, w, eps, int(clamp), om,
+                   logit, mean, rstd, device=y.device)
         ctx.save_for_backward(y, keep, b_e, gamma, beta, u, c, mean, rstd)
         ctx.clamp = int(clamp)
         return om, logit
 
     @staticmethod
     def backward(ctx, g_om, g_logit):
-        from uninext_b200 import _cabi
-        lib = _cabi.twostage()
         y, keep, b_e, gamma, beta, u, c, mean, rstd = ctx.saved_tensors
         n, s, w = y.shape
         g_om, g_logit = g_om.contiguous(), g_logit.contiguous()
         g_y = torch.empty_like(y)
         g_be, g_gamma, g_beta = torch.empty_like(b_e), torch.empty_like(gamma), torch.empty_like(beta)
         g_u, g_c = torch.empty_like(u), torch.empty_like(c)
-        nbytes = ctypes.c_int64()
-        _cabi.check(lib.msda_twostage_head_workspace(n, s, w, ctypes.byref(nbytes)), "msda_twostage_head_workspace")
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=y.device)
-        _cabi.check(lib.msda_twostage_head_backward_f32(
-            g_om.data_ptr(), g_logit.data_ptr(), y.data_ptr(), keep.data_ptr(), b_e.data_ptr(), gamma.data_ptr(),
-            beta.data_ptr(), u.data_ptr(), c.data_ptr(), mean.data_ptr(), rstd.data_ptr(), n, s, w, ctx.clamp, g_y.data_ptr(),
-            g_be.data_ptr(), g_gamma.data_ptr(), g_beta.data_ptr(), g_u.data_ptr(), g_c.data_ptr(), ws.data_ptr(),
-            nbytes.value, _stream()), "msda_twostage_head_backward_f32")
+        nbytes = _cabi.workspace("msda_twostage_head_workspace", n, s, w)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
+        _cabi.call("msda_twostage_head_backward_f32", g_om, g_logit, y, keep, b_e, gamma, beta, u, c, mean, rstd, n, s,
+                   w, ctx.clamp, g_y, g_be, g_gamma, g_beta, g_u, g_c, ws, nbytes, device=y.device)
         return g_y, None, g_be, g_gamma, g_beta, g_u, g_c, None, None
 
 
@@ -122,18 +109,14 @@ class _Select(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, box, proposals, logit, k):
-        from uninext_b200 import _cabi
-        lib = _cabi.twostage()
         n, s, _ = box.shape
         coord = torch.empty_like(box)
         ref = box.new_empty((n, k, 4))
         idx = torch.empty((n, k), dtype=torch.int64, device=box.device)
-        nbytes = ctypes.c_int64()
-        _cabi.check(lib.msda_twostage_select_workspace(n, s, k, ctypes.byref(nbytes)), "msda_twostage_select_workspace")
-        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=box.device)
-        _cabi.check(lib.msda_twostage_select_forward_f32(logit.data_ptr(), box.data_ptr(), proposals.data_ptr(), n, s, k,
-                                                         coord.data_ptr(), ref.data_ptr(), idx.data_ptr(), ws.data_ptr(),
-                                                         nbytes.value, _stream()), "msda_twostage_select_forward_f32")
+        nbytes = _cabi.workspace("msda_twostage_select_workspace", n, s, k)
+        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=box.device)
+        _cabi.call("msda_twostage_select_forward_f32", logit, box, proposals, n, s, k, coord, ref, idx, ws, nbytes,
+                   device=box.device)
         ctx.save_for_backward(ref, idx)
         ctx.mark_non_differentiable(idx)
         ctx.sizes = (n, s, k)
@@ -141,14 +124,11 @@ class _Select(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_coord, g_ref, _g_idx):
-        from uninext_b200 import _cabi
-        lib = _cabi.twostage()
         ref, idx = ctx.saved_tensors
         n, s, k = ctx.sizes
         g_box = g_coord.contiguous().clone()              # the kernel adds the selected rows' gradient in place
-        _cabi.check(lib.msda_twostage_select_backward_f32(g_ref.contiguous().data_ptr(), ref.data_ptr(), idx.data_ptr(), n,
-                                                          s, k, g_box.data_ptr(), _stream()),
-                    "msda_twostage_select_backward_f32")
+        _cabi.call("msda_twostage_select_backward_f32", g_ref.contiguous(), ref, idx, n, s, k, g_box,
+                   device=g_box.device)
         return g_box, None, None, None
 
 
@@ -194,7 +174,7 @@ def two_stage_select(memory, memory_padding_mask, spatial_shapes, enc_output, en
         topk_coords_unact = torch.gather(enc_outputs_coord_unact, 1, topk_proposals.unsqueeze(-1).repeat(1, 1, 4))
         return enc_outputs_class, enc_outputs_coord_unact, topk_coords_unact.sigmoid(), topk_proposals
     _check_cuda(memory, enc_output, enc_output_norm, class_embed)
-    with torch.cuda.device(memory.device), torch.autocast("cuda", enabled=False):
+    with torch.autocast("cuda", enabled=False):
         y = F.linear(memory, enc_output.weight, enc_output.bias)
         u, c, clamp = class_embed.logit_affine(n, lang_feat_pool)
         u, c = u.float().contiguous(), c.float().reshape(n).contiguous()

@@ -13,8 +13,6 @@ limits (head_dim 128 / 256, T <= 256).
 """
 from __future__ import annotations
 
-import ctypes
-
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -77,19 +75,9 @@ def fused_supported(q, k, stable_softmax_2d=False, vv=None, vl=None) -> bool:
             and q.shape[-1] in HEAD_DIMS and 1 <= k.shape[1] <= MAX_TEXT_TOKENS and q.shape[1] >= 1)
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _workspace(B, H, S, T, D, device):
-    lib = _cabi.load()
-    n = ctypes.c_int64(0)
-    _cabi.check(lib.msda_vlfuse_workspace(B, H, S, T, D, ctypes.byref(n)), "msda_vlfuse_workspace")
-    return torch.empty(max(n.value, 16), dtype=torch.uint8, device=device)
+    n = _cabi.workspace("msda_vlfuse_workspace", B, H, S, T, D)
+    return torch.empty(max(n, 16), dtype=torch.uint8, device=device)
 
 
 def draw_seed(device):
@@ -102,8 +90,7 @@ def dropout_masks(seed, B, H, S, T, p):
     """The keep-masks (1.0 / 0.0) the kernels apply for this seed: vision [B, H, S, T], text [B, H, T, S]."""
     mv = torch.empty(B, H, S, T, dtype=torch.float32, device=seed.device)
     ml = torch.empty(B, H, T, S, dtype=torch.float32, device=seed.device)
-    _cabi.check(_cabi.load().msda_vlfuse_dropout_mask_f32(_ptr(seed), B, H, S, T, ctypes.c_float(p), _ptr(mv), _ptr(ml),
-                                                          _stream()), "msda_vlfuse_dropout_mask_f32")
+    _cabi.call("msda_vlfuse_dropout_mask_f32", seed, B, H, S, T, float(p), mv, ml, device=seed.device)
     return mv, ml
 
 
@@ -124,11 +111,8 @@ class VLAttentionFunction(torch.autograd.Function):
         o_l = torch.empty_like(k)
         stats = torch.empty(B * H * (S + T) * 2, dtype=torch.float32, device=q.device)
         ws = _workspace(B, H, S, T, D, q.device)
-        name = f"msda_vlfuse_forward_{mode}"
-        _cabi.check(getattr(_cabi.load(), name)(
-            _ptr(q), _ptr(k), _ptr(vv), _ptr(vl), _ptr(bias), B, H, S, T, D, int(clamp_min), int(clamp_max),
-            ctypes.c_float(dropout_p), _ptr(seed), _ptr(o_v), _ptr(o_l), _ptr(stats), _ptr(ws), ws.numel(), _stream()),
-            name)
+        _cabi.call(f"msda_vlfuse_forward_{mode}", q, k, vv, vl, bias, B, H, S, T, D, int(clamp_min), int(clamp_max),
+                   float(dropout_p), seed, o_v, o_l, stats, ws, ws.numel(), device=q.device)
         ctx.save_for_backward(q, k, vv, vl, bias, seed, o_v, o_l, stats)
         ctx.cfg = (clamp_min, clamp_max, dropout_p, mode)
         return o_v, o_l
@@ -143,11 +127,9 @@ class VLAttentionFunction(torch.autograd.Function):
         go_l = torch.zeros_like(o_l) if go_l is None else go_l.contiguous()
         dq, dk, dvv, dvl = (torch.empty_like(t) for t in (q, k, vv, vl))
         ws = _workspace(B, H, S, T, D, q.device)
-        name = f"msda_vlfuse_backward_{mode}"
-        _cabi.check(getattr(_cabi.load(), name)(
-            _ptr(go_v), _ptr(go_l), _ptr(q), _ptr(k), _ptr(vv), _ptr(vl), _ptr(bias), _ptr(o_v), _ptr(o_l), _ptr(stats),
-            B, H, S, T, D, int(clamp_min), int(clamp_max), ctypes.c_float(dropout_p), _ptr(seed), _ptr(dq), _ptr(dk),
-            _ptr(dvv), _ptr(dvl), _ptr(ws), ws.numel(), _stream()), name)
+        _cabi.call(f"msda_vlfuse_backward_{mode}", go_v, go_l, q, k, vv, vl, bias, o_v, o_l, stats, B, H, S, T, D,
+                   int(clamp_min), int(clamp_max), float(dropout_p), seed, dq, dk, dvv, dvl, ws, ws.numel(),
+                   device=q.device)
         return dq, dk, dvv, dvl, None, None, None, None, None, None
 
 
