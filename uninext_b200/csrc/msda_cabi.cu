@@ -144,9 +144,9 @@ template <typename T> struct FwdVec { static constexpr int v = 16 / sizeof(T); }
 template <typename T> struct BwdVec { static constexpr int v = 4; };                  // 4 channels per lane (see RowVec)
 
 // Launch of a kernel of kTiledThreads threads.  pdl: the kernel just issued on `st` is the programmatic-dependent-launch
-// primary (the grad_value zero-fill, as zero_fill reported it, or the region backward's tap kernel): the kernel's
-// prologue overlaps the primary, and the kernel must wait for it (pdl_wait_primary) before touching grad_value.  Only the
-// backward kernels that do so take `pdl`.
+// primary (the grad_value zero-fill, as zero_fill reported it, or the region backward's grad_value kernel): the kernel's
+// prologue overlaps the primary, and the kernel must wait for it (pdl_wait_primary) before touching grad_value, or, the
+// region tap kernel, before it exits.  Only the backward kernels that do so take `pdl`.
 template <typename K, typename... Args>
 cudaError_t launch_after_fill(K kern, int grid, size_t smem, cudaStream_t st, bool pdl, Args... args) {
     if (pdl) {
@@ -331,35 +331,39 @@ bool use_region(const Dims &d) {
            !use_split(num_pairs(d));
 }
 
-// Two launches: the tap kernel (grad_loc / grad_attn), a PDL secondary of the zero-fill when `pdl`, then the grad_value
-// kernel, a PDL secondary of the tap kernel whenever the stream is not capturing (msda_region.cuh: the chain is
-// transitive).  Under capture the grad_value kernel follows in plain stream order.
+// Two launches: the grad_value kernel, a PDL secondary of the zero-fill when `pdl`, then the tap kernel (grad_loc /
+// grad_attn), a PDL secondary of the grad_value kernel whenever the stream is not capturing, so that its CTAs run beside
+// the grad_value CTAs (msda_region.cuh: the chain is transitive).  Under capture the tap kernel follows in plain stream
+// order.
 cudaError_t launch_bwd_region(const float *go, const float *value, const int64_t *shapes, const int64_t *lsi,
                               const float *loc, const float *attn, const Dims &d, float *gv, float *gl, float *ga,
                               bool pdl, cudaStream_t st) {
     constexpr auto tap = msda::msda_bwd_region<msda::kRegionEdge, msda::kRegionHalo>;
     constexpr auto gvk = msda::msda_region_grad_value_pass<msda::kRegionEdge, msda::kRegionHalo>;
     constexpr size_t tap_smem = msda::region_tap_smem_bytes(), gv_smem = msda::region_gv_smem_bytes();
-    if (const cudaError_t e = opt_in_smem<gvk>((int)gv_smem)) return e;
-    const auto resident = [](auto kern, size_t smem) {
-        int per_sm = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, msda::kTiledThreads, smem) != cudaSuccess || per_sm < 1)
-            per_sm = 1;
-        return per_sm * num_sms();
-    };
-    static PerDevice<int> tap_slots, gv_slots;
-    const int tap_grid = tap_slots.get([&](int) { return resident(tap, tap_smem); });
-    const int gv_grid = gv_slots.get([&](int) { return resident(gvk, gv_smem); });
+    static PerDevice<int> ready;
+    static msda::RegionGrids grids[kMaxDevices];
+    cudaError_t e = cudaSuccess;
+    const int dev = current_device();
+    ready.get([&](int dv) {
+        if ((e = cudaFuncSetAttribute(gvk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gv_smem)) != cudaSuccess)
+            return 0;
+        grids[dv] = msda::region_grids(gvk, gv_smem, tap, tap_smem, num_sms());
+        return 1;
+    });
+    if (e != cudaSuccess) return e;
+    const msda::RegionGrids &rg = grids[dev];
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    const bool chain = cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     const unsigned npairs = num_pairs(d);
     const int tma = use_tma_staging(d) ? 1 : 0;            // the tap pass: TMA-staged or __ldg taps, as msda_bwd_tiled
     g_launches.fetch_add(2, std::memory_order_relaxed);
-    cudaError_t e = launch_after_fill(tap, tap_grid, tap_smem, st, pdl, go, value, shapes, lsi, loc, attn, d.N, d.S, d.M,
-                                      d.L, d.Lq, d.P, npairs, tma, gl, ga);
+    // Under capture the two kernels run one after the other, each at its own occupancy and unpadded.
+    e = launch_after_fill(gvk, chain ? rg.gv : rg.gv_solo, chain ? rg.gv_smem : gv_smem, st, pdl, go, shapes, lsi, loc,
+                          attn, d.N, d.S, d.M, d.L, d.Lq, d.P, npairs, gv);
     if (e != cudaSuccess) return e;
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    const bool chain = cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
-    return launch_after_fill(gvk, gv_grid, gv_smem, st, chain, go, shapes, lsi, loc, attn, d.N, d.S, d.M, d.L, d.Lq, d.P,
-                             npairs, gv);
+    return launch_after_fill(tap, chain ? rg.tap : rg.tap_solo, tap_smem, st, chain, go, value, shapes, lsi, loc, attn, d.N,
+                             d.S, d.M, d.L, d.Lq, d.P, npairs, tma, gl, ga);
 }
 
 template <typename T>

@@ -12,7 +12,7 @@
 //   msda_bwd_region (tap pass, 2 CTAs/SM): msda_bwd_tiled's NORED body (linear chunks of pairs, taps TMA-staged one
 //             iteration ahead when L*P % 4 == 0): the gathers, grad_loc and grad_attn, from the same device code and in
 //             the same FMA order as msda_bwd_tiled.
-//   msda_region_grad_value_pass (3 CTAs/SM), per tile = (b, m, region).  A query at pixel (x, y) of level l belongs to
+//   msda_region_grad_value_pass (__launch_bounds__ for 3 CTAs/SM), per tile = (b, m, region).  A query at pixel (x, y) of level l belongs to
 //             region floor((x + 0.5) * Wref / W_l / R) in x (likewise in y; Wref / Href = the largest level), so a
 //             region holds one contiguous x-range and y-range per level, in closed form.  The window on level l is the
 //             region scaled to level l plus kRegionHalo pixels.
@@ -24,9 +24,13 @@
 //     phase B: scan of the row counts, then scatter of the entry indices by window row (integer shared atomics only:
 //              fp32 shared atomics are CAS loops) into one u16 array.
 //     phase C: one group per touched row sums coefficient x stashed grad_out in registers and issues one red per lane.
-// PDL chain: zero-fill (primary) -> tap kernel -> grad_value kernel.  The tap kernel writes nothing the fill writes, so it
-// lets its dependent launch at once and waits for the fill as its last statement: its completion then implies the fill's,
-// and the grad_value kernel, which waits for the tap kernel before its first red, sees a zeroed grad_value.
+// The two kernels share no data (the tap pass writes grad_loc / grad_attn, the grad_value pass grad_value), and they are
+// limited by different things: the tap pass by its gathers, the grad_value pass by latency.  So they run side by side on
+// every SM, 2 grad_value CTAs beside 1 tap CTA (the host sizes both grids for that), chained by PDL:
+//   zero-fill (primary) -> grad_value kernel -> tap kernel.
+// The grad_value kernel lets its dependent launch at once, so the tap CTAs fill the room its CTAs leave, and waits for the
+// fill before its first red (and, if it had none, before it exits).  The tap kernel waits for the grad_value kernel as its
+// last statement: its completion then implies the grad_value kernel's and, through it, the fill's.
 // A level table that does not tile [0, S) (the patch-order condition) runs the grad_value pass in linear chunks of pairs
 // with no window: every corner reds directly.
 #pragma once
@@ -43,8 +47,10 @@ constexpr int kRegionWinRows = 1024;      // window rows per tile (levels past t
 // (tests/region_layout.py) reads it.
 constexpr int kRegionStageRows = 384;
 constexpr int kRegionEntries = kRegionSlots * 16 * 4;   // one entry position per (slot, tap, corner); L*P <= 16
+// __launch_bounds__ minimum CTAs per SM.  They fix each kernel's register budget; the grids are sized on the host
+// (2 grad_value CTAs + 1 tap CTA per SM on an H100).
 constexpr int kRegionTapCtas = 2;         // tap kernel: it needs 128 registers per thread
-constexpr int kRegionGvCtas = 3;          // grad_value kernel: latency-bound, so as many resident warps as fit
+constexpr int kRegionGvCtas = 3;          // grad_value kernel: latency-bound, 46 registers
 constexpr int kRegionIterSlots = kTiledWarps * 4;       // pairs per CTA iteration (D = 32: 4 groups of 8 lanes per warp)
 
 // The tap kernel's TMA stage buffers (kTiledWarps per-warp double buffers of one iteration's (x, y, a)).
@@ -83,6 +89,31 @@ __device__ int g_region_knockout;
 #define MSDA_REGION_KEEP_RED(bit) true
 #endif
 
+#ifdef MSDA_REGION_COSCHED
+// Placement hook for tools/region_cosched.py; the library build never defines it.  Thread 0 of each CTA of kernel k
+// (0 = grad_value, 1 = tap) writes {%smid, %globaltimer at its start, %globaltimer when its work is done} into
+// g_region_cosched[k][3 * blockIdx.x ...], the end after a CTA barrier (and, in the tap kernel, before its PDL wait).
+__device__ unsigned long long *g_region_cosched[2];
+__device__ __forceinline__ unsigned long long region_globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+#define MSDA_REGION_COSCHED_START(k)                                                               \
+    if (threadIdx.x == 0) {                                                                        \
+        unsigned smid;                                                                             \
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));                                         \
+        g_region_cosched[k][3 * blockIdx.x] = smid;                                                \
+        g_region_cosched[k][3 * blockIdx.x + 1] = region_globaltimer();                            \
+    }
+#define MSDA_REGION_COSCHED_END(k)                                                                 \
+    __syncthreads();                                                                               \
+    if (threadIdx.x == 0) g_region_cosched[k][3 * blockIdx.x + 2] = region_globaltimer();
+#else
+#define MSDA_REGION_COSCHED_START(k)
+#define MSDA_REGION_COSCHED_END(k)
+#endif
+
 struct RegionMap {
     int H[kMaxLevels], W[kMaxLevels], start[kMaxLevels];
     int Href, Wref, nry, nrx;
@@ -103,9 +134,8 @@ __device__ __forceinline__ int region_first(int r, int n, int ref, int R) {
     return num <= 0 ? 0 : (int)min((long long)n, (num + 2ll * ref - 1) / (2ll * ref));
 }
 
-// The grad_value pass, a persistent PDL secondary of the tap kernel (msda_bwd_region).  Its first tile's geometry and
-// entries overlap the tap kernel's last wave; it waits for the tap kernel, and through it for the zero-fill, before its
-// first red.
+// The grad_value pass, a persistent PDL secondary of the zero-fill and the PDL primary of the tap kernel
+// (msda_bwd_region).  It waits for the fill before its first red; its first tile's geometry and entries overlap the fill.
 template <int R, int HALO>
 __global__ void __launch_bounds__(kTiledThreads, kRegionGvCtas)
 msda_region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *__restrict__ shapes,
@@ -129,6 +159,8 @@ msda_region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *_
     unsigned short *e_row = reinterpret_cast<unsigned short *>(cnt + kRegionWinRows); // [slot][tap][corner], kNoRow = none
     unsigned short *s_idx = e_row + kRegionEntries;     // phases B, C: entry indices sorted by window row
 
+    pdl_launch_dependents();     // the tap kernel's CTAs may take the room this kernel leaves on each SM
+    MSDA_REGION_COSCHED_START(0);
     MSDA_REGION_CLOCK_INIT;
     if (threadIdx.x == 0) {            // the map comes from the device-resident level table: no host read, capture-safe
         int run = 0, href = 0, wref = 0;
@@ -272,7 +304,7 @@ msda_region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *_
             }
 
             // ---- direct reds: the group walks the taps of its pair that have a corner to red ----
-            if (!primary_done) {       // the tap kernel, and so grad_value's zero-fill, are complete and visible
+            if (!primary_done) {       // grad_value's zero-fill is complete and visible
                 pdl_wait_primary();
                 primary_done = true;
             }
@@ -364,6 +396,9 @@ msda_region_grad_value_pass(const float *__restrict__ grad_out, const int64_t *_
         __syncthreads();              // the next tile rewrites tl, the entry list, the stash and the counts
         MSDA_REGION_CLOCK(nwin > 0 ? 3 : 1);
     }
+    // The tap kernel takes this kernel's completion to imply the fill's, so a CTA that issued no red waits here.
+    if (!primary_done) pdl_wait_primary();
+    MSDA_REGION_COSCHED_END(0);
 }
 
 // The tap pass: grad_loc / grad_attn.  tma: it stages (x, y, a) with TMA (use_tma_staging on the host: L*P % 4 == 0).
@@ -380,7 +415,7 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
     __shared__ __align__(8) unsigned long long stage_bar[kTiledWarps * 2];
     extern __shared__ __align__(128) unsigned char stage_mem[];        // region_tap_smem_bytes()
 
-    pdl_launch_dependents();     // the grad_value kernel's prologue may run on SM slots this kernel frees
+    MSDA_REGION_COSCHED_START(1);
     if (tma)
         bwd_tiled_body<float, 4, 32, 16, true, false, false, true, false>(
             wm, slab_mem, stage_mem, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
@@ -389,9 +424,68 @@ msda_bwd_region(const float *__restrict__ grad_out, const float *__restrict__ va
         bwd_tiled_body<float, 4, 32, 16, false, false, false, true, false>(
             wm, slab_mem, stage_mem, stage_bar, grad_out, value, shapes, lsi, loc, attn, N, S, M, L, Lq, P, npairs, 0,
             nullptr, grad_loc, grad_attn, nullptr, 0);
-    // Nothing here writes what the zero-fill writes, but the grad_value kernel relies on this kernel's completion
-    // implying the fill's: wait for the PDL primary last.
+    MSDA_REGION_COSCHED_END(1);
+    // Nothing here touches grad_value, but the next operation on the stream relies on this kernel's completion implying
+    // the grad_value kernel's (and the fill's): wait for the PDL primary last.
     pdl_wait_primary();
+}
+
+// Launch sizes of the region backward's two kernels.  Side by side (the PDL chain): the most grad_value CTAs per SM, g (at
+// most its own occupancy), that leave room for one tap CTA in the SM's registers (allocated per warp in units of 256),
+// shared memory (static + dynamic + the per-CTA reservation) and threads; on an H100 that is 2 + 1, 2 x 12 288 + 32 768
+// registers.  The block scheduler places a kernel's CTAs wherever they fit, so if g + 1 grad_value CTAs fit an SM it puts
+// g + 1 on some SMs and none on others, and two tap CTAs then run alone there.  The grad_value kernel's dynamic shared
+// memory is therefore padded until g + 1 no longer fit, and it asks for the largest shared-memory carveout, so that the
+// SM keeps room for the tap CTA.  Alone (no chain, or where no grad_value CTA fits beside a tap CTA) each kernel gets its
+// own occupancy.  Host code, shared by the library and tools/region_cosched.cu; the caller has opted the grad_value
+// kernel in to gv_smem bytes of dynamic shared memory.
+struct RegionGrids {
+    int gv, tap;                // side by side: grids
+    size_t gv_smem;             // side by side: the grad_value kernel's (padded) dynamic shared memory
+    int gv_solo, tap_solo;      // one after the other: grids
+};
+
+template <class GV, class TAP>
+RegionGrids region_grids(GV gvk, size_t gv_smem, TAP tap, size_t tap_smem, int sms) {
+    const auto occupancy = [](auto kern, size_t smem) {
+        int per_sm = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kTiledThreads, smem) != cudaSuccess || per_sm < 1)
+            per_sm = 1;
+        return per_sm;
+    };
+    const int gv_occ = occupancy(gvk, gv_smem), tap_occ = occupancy(tap, tap_smem);
+    const RegionGrids solo = {gv_occ * sms, tap_occ * sms, gv_smem, gv_occ * sms, tap_occ * sms};
+    int dev = 0, regs_sm = 0, smem_sm = 0, smem_optin = 0, reserved = 0, threads_sm = 0;
+    cudaFuncAttributes ga{}, ta{};
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&regs_sm, cudaDevAttrMaxRegistersPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&threads_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev) != cudaSuccess ||
+        cudaFuncGetAttributes(&ga, gvk) != cudaSuccess || cudaFuncGetAttributes(&ta, tap) != cudaSuccess)
+        return solo;
+    constexpr int warps = kTiledThreads / 32;
+    const auto regs = [](int per_thread) { return warps * ((per_thread * 32 + 255) / 256 * 256); };
+    const auto smem = [&](const cudaFuncAttributes &a, size_t dyn) { return (long long)a.sharedSizeBytes + (long long)dyn + reserved; };
+    for (int g = gv_occ; g >= 1; --g) {
+        size_t dyn = gv_smem;
+        if (g < gv_occ) {           // pad in 1 KB steps until g + 1 CTAs exceed the SM
+            const long long over = (long long)smem_sm / (g + 1) + 1 - smem(ga, 0);
+            dyn = (size_t)((over + 1023) / 1024 * 1024);
+        }
+        if ((long long)g * regs(ga.numRegs) + regs(ta.numRegs) <= regs_sm && (long long)dyn <= smem_optin &&
+            g * smem(ga, dyn) + smem(ta, tap_smem) <= smem_sm && (g + 1) * kTiledThreads <= threads_sm) {
+            if (dyn != gv_smem &&
+                (cudaFuncSetAttribute(gvk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess ||
+                 cudaFuncSetAttribute(gvk, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                      (int)cudaSharedmemCarveoutMaxShared) != cudaSuccess ||
+                 occupancy(gvk, dyn) != g))
+                return solo;
+            return {g * sms, sms, dyn, solo.gv_solo, solo.tap_solo};
+        }
+    }
+    return solo;
 }
 
 }  // namespace msda
