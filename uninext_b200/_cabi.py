@@ -88,6 +88,13 @@ FLATTEN_SIGNATURES = {
     "msda_flatten_levels_workspace": (_i, [_vp] * 2 + [_i] * 3 + [_vp]),
     "msda_flatten_levels_backward_f32": (_i, [_vp] * 4 + [_i] * 3 + [_vp] * 4 + [_i64, _vp]),
 }
+# Typed by entry() on first use rather than by load(), so a library without them leaves load().missing as it was: the
+# video trackers' detection selection (include/msda_trackpost.h).
+TRACKPOST_SIGNATURES = {
+    "msda_trackpost_workspace": (_i, [_i] * 4 + [_vp]),
+    "msda_trackpost_f32": (_i, [_vp] * 6 + [_i] * 4 + [ctypes.c_float] * 2 + [_i] + [_vp] * 5 + [_vp, _i64, _vp]),
+}
+TRACKPOST_CXCYWH, TRACKPOST_XYXY_PIXELS = 0, 1                                                         # include/msda_trackpost.h
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
 
@@ -141,10 +148,13 @@ def entry(name: str, path: str | None = None):
     fn = _entries.get(name) if path is None else None
     if fn is None:
         lib = load(path)
-        if name in lib.missing:
+        late = TRACKPOST_SIGNATURES.get(name)
+        if name in lib.missing or (late and not hasattr(lib, name)):
             raise MSDALibraryError(f"{path or LIB_PATH} does not export `{name}` (stale build? run "
                                    "uninext_b200.build --force)")
         fn = getattr(lib, name)
+        if late:
+            fn.restype, fn.argtypes = late
         if path is None:
             _entries[name] = fn
     return fn
@@ -164,6 +174,11 @@ def twostage(path: str | None = None):
 def flatten(path: str | None = None):
     """The library, after checking that it exports the input preparation (include/msda_flatten.h)."""
     return _with_group(FLATTEN_SIGNATURES, path)
+
+
+def trackpost(path: str | None = None):
+    """The library, after checking that it exports the trackers' detection selection (include/msda_trackpost.h)."""
+    return _with_group(TRACKPOST_SIGNATURES, path)
 
 
 def call(name: str, *args, device) -> None:

@@ -1,6 +1,8 @@
 // msda_cabi_postprocess.cu -- C ABI of the inference post-processing: mask pasting (msda_maskpaste.cuh), COCO run-length
-// encoding of masks (msda_maskrle.cuh) and detection post-processing (msda_detpost.cuh).
+// encoding of masks (msda_maskrle.cuh), detection post-processing and the video trackers' detection selection
+// (msda_detpost.cuh; the latter's entry points are declared in include/msda_trackpost.h).
 #include "../../include/msda_b200.h"
+#include "../../include/msda_trackpost.h"
 #include "msda_detpost.cuh"
 #include "msda_host.cuh"
 #include "msda_maskpaste.cuh"
@@ -166,6 +168,44 @@ int msda_detpost_f32(const float *box_cls, const float *box_pred, const float *i
     }
     g_launches.fetch_add(2, std::memory_order_relaxed);
     return (int)cudaGetLastError();
+}
+
+int msda_trackpost_workspace(int B, int Q, int T, int C, int64_t *bytes) {
+    if (!bytes) return MSDA_E_BADARG;
+    if (const int c = detpost_check(B, Q, T, C, 1)) return c;
+    *bytes = (int64_t)detpost_layout(B, Q, C, 1).total;        // prob, qmax, qarg; one result needs no sort buffer
+    return 0;
+}
+
+int msda_trackpost_f32(const float *box_cls, const float *box_pred, const float *iou_pred, const int *class_start,
+                       const int *tokens, const int *ori_sizes, int B, int Q, int T, int C, float score_thres,
+                       float nms_iou, int box_format, float *scores, int *labels, int *query_index, float *boxes,
+                       int *count, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (box_format != MSDA_TRACKPOST_CXCYWH && box_format != MSDA_TRACKPOST_XYXY_PIXELS) return MSDA_E_BADARG;
+    const bool pixels = box_format == MSDA_TRACKPOST_XYXY_PIXELS;
+    if (!box_cls || !box_pred || !class_start || !tokens || (pixels && !ori_sizes) || !scores || !labels ||
+        !query_index || !boxes || !count || !workspace || !aligned16(boxes) || !aligned16(workspace))
+        return MSDA_E_BADARG;
+    if (const int c = detpost_check(B, Q, T, C, 1)) return c;
+    const DetpostLayout l = detpost_layout(B, Q, C, 1);
+    if (workspace_bytes < (int64_t)l.total) return MSDA_E_BADARG;
+    if (B == 0) return 0;
+    char *ws = static_cast<char *>(workspace);
+    float *prob = reinterpret_cast<float *>(ws + l.prob), *qmax = reinterpret_cast<float *>(ws + l.qmax);
+    int *qarg = reinterpret_cast<int *>(ws + l.qarg);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 sgrid((unsigned)((Q + msda::kDpScoreWarps - 1) / msda::kDpScoreWarps), (unsigned)B);
+    if (const cudaError_t e = launch(msda::detpost_scores, sgrid, msda::kDpScoreWarps * 32, 0, st, box_cls, iou_pred,
+                                     class_start, tokens, Q, T, C, prob, qmax, qarg))
+        return (int)e;
+    // The opt-in is set once per device, to the Q = kDpMaxQ size, as for detpost_select<true>.
+    constexpr int kDynMax = msda::kDpMaxQ * (int)sizeof(float4) +
+                            msda::kDpMaxQ * ((msda::kDpMaxQ + 63) / 64) * (int)sizeof(unsigned long long);
+    if (const cudaError_t e = opt_in_smem<msda::trackpost_select>(kDynMax)) return (int)e;
+    const size_t dyn = (size_t)Q * sizeof(float4) + (size_t)Q * ((Q + 63) / 64) * sizeof(unsigned long long);
+    return (int)launch(msda::trackpost_select, dim3((unsigned)B), msda::kDpThreads, dyn, st, box_pred,
+                       pixels ? ori_sizes : nullptr, qmax, qarg, Q, score_thres, nms_iou, (int)pixels, scores, labels,
+                       query_index, boxes, count);
 }
 
 int msda_mask_rle_workspace(int64_t I, int out_h, int out_w, int64_t *bytes) {

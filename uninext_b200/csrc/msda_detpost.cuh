@@ -13,11 +13,17 @@
 //   detpost_select   one CTA per image: [NMS: stable rank sort of the Q maxima, the Q x ceil(Q/64) IoU bitmask in shared
 //                    memory, the greedy sweep in one warp,] then a radix select of the top `count` of the K*C candidates
 //                    on a unique 64-bit key (value, flat index), a bitonic sort of those, and the outputs.
+// The video trackers' per-frame selection (uninext_vid.py:1224-1250 MOT, :1380-1415 VIS; DESIGN.md section 3.17) is two
+// launches as well: detpost_scores, then
+//   trackpost_select one CTA per frame: the candidates max_score > score_thres compacted in query order, [none: the
+//                    query of the largest max_score; else: the stable rank sort of the candidates, the bitmask and the
+//                    sweep (msda_nms.cuh) on the compacted set,] then the kept queries in keep order.
 // Every multiply and add is written with __fmul_rn / __fadd_rn / __fsub_rn so that nvcc does not contract it into an
 // FMA: the contract is this uncontracted arithmetic (DESIGN.md section 3.13).
 #pragma once
 
 #include "msda_common.cuh"
+#include "msda_nms.cuh"
 #include "msda_topk.cuh"
 
 namespace msda {
@@ -71,22 +77,11 @@ detpost_scores(const float *__restrict__ box_cls, const float *__restrict__ iou_
 }
 
 // box_cxcywh_to_xyxy: (x_c - 0.5 * w, y_c - 0.5 * h, x_c + 0.5 * w, y_c + 0.5 * h), each operation rounded once.
-__device__ __forceinline__ float4 dp_xyxy(const float *b) {
-    const float cx = __ldg(b), cy = __ldg(b + 1), hw = __fmul_rn(0.5f, __ldg(b + 2)), hh = __fmul_rn(0.5f, __ldg(b + 3));
+__device__ __forceinline__ float4 dp_xyxy(float cx, float cy, float w, float h) {
+    const float hw = __fmul_rn(0.5f, w), hh = __fmul_rn(0.5f, h);
     return make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
 }
-
-// The expression of torchvision's devIoU (ops/cuda/nms_kernel.cu) with every operation rounded once.  torchvision's
-// build may contract parts of it into FMAs, so the two can differ in the last bit of the IoU.
-__device__ __forceinline__ bool dp_iou_above(float4 a, float4 b, float thr) {
-    const float left = fmaxf(a.x, b.x), right = fminf(a.z, b.z);
-    const float top = fmaxf(a.y, b.y), bottom = fminf(a.w, b.w);
-    const float width = fmaxf(__fsub_rn(right, left), 0.f), height = fmaxf(__fsub_rn(bottom, top), 0.f);
-    const float inter = __fmul_rn(width, height);
-    const float sa = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
-    const float sb = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
-    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(sa, sb), inter)) > thr;
-}
+__device__ __forceinline__ float4 dp_xyxy(const float *b) { return dp_xyxy(__ldg(b), __ldg(b + 1), __ldg(b + 2), __ldg(b + 3)); }
 
 __device__ __forceinline__ float dp_block_max(float v, float *red) {
 #pragma unroll
@@ -122,7 +117,6 @@ detpost_select(const float *__restrict__ box_pred, const int *__restrict__ image
     int K = Q;
     if constexpr (NMS) {
         float4 *sbox = dp_dyn;
-        const int W = (Q + 63) / 64;
         unsigned long long *mask = reinterpret_cast<unsigned long long *>(sbox + Q);
         const float *qm = qmax + (size_t)b * Q;
         // batched_nms's coordinate trick: m = boxes.max(), offset = class * (m + 1) added to each coordinate
@@ -147,32 +141,10 @@ detpost_select(const float *__restrict__ box_pred, const int *__restrict__ image
             s_keep[rank] = i;                   // s_keep holds the sorted order until the sweep compacts it
         }
         __syncthreads();
-        for (int it = tid; it < Q * W; it += kDpThreads) {
-            const int i = it / W, w = it - i * W;
-            unsigned long long bits = 0;
-            const int j0 = max(w * 64, i + 1), j1 = min(w * 64 + 64, Q);
-            if (j0 < j1) {
-                const float4 a = sbox[i];
-                for (int j = j0; j < j1; ++j)
-                    if (dp_iou_above(a, sbox[j], nms_iou)) bits |= 1ull << (j - w * 64);
-            }
-            mask[it] = bits;
-        }
+        nms_bitmask<kDpThreads>(sbox, Q, nms_iou, mask);
         __syncthreads();
-        if (tid < 32) {                         // greedy sweep: lane l holds removed-word l (W <= 16)
-            unsigned long long removed = 0;
-            int k = 0;
-            for (int i = 0; i < Q; ++i) {
-                const unsigned long long word = __shfl_sync(0xffffffffu, removed, i >> 6);
-                if (!((word >> (i & 63)) & 1ull)) {
-                    const int qi = s_keep[i];   // read before any lane overwrites slot k <= i
-                    __syncwarp();
-                    if (tid == 0) s_keep[k] = qi;
-                    ++k;
-                    if (tid < W) removed |= mask[(size_t)i * W + tid];
-                }
-                __syncwarp();
-            }
+        if (tid < 32) {
+            const int k = nms_sweep(mask, Q, s_keep);
             if (tid == 0) s_K = k;
         }
         __syncthreads();
@@ -223,6 +195,111 @@ detpost_select(const float *__restrict__ box_pred, const int *__restrict__ image
         }
     }
     if (tid == 0) count[b] = (int)cnt;
+}
+
+// One CTA per frame (grid = B), thread i <-> query i (Q <= kDpThreads).  Dynamic shared memory as detpost_select<true>'s
+// for Q queries, of which the n candidates use float4 boxes[n] in score order and the bitmask u64 mask[n][ceil(n/64)].
+// pixels: boxes are box_cxcywh_to_xyxy of the cxcywh box scaled by (W, H, W, H) of ori_sizes[b] = (H, W); else the
+// normalised cxcywh box as it is.
+__global__ void __launch_bounds__(kDpThreads, 1)
+trackpost_select(const float *__restrict__ box_pred, const int *__restrict__ ori_sizes, const float *__restrict__ qmax,
+                 const int *__restrict__ qarg, int Q, float score_thres, float nms_iou, int pixels,
+                 float *__restrict__ scores, int *__restrict__ labels, int *__restrict__ query_index,
+                 float *__restrict__ boxes, int *__restrict__ count)
+{
+    extern __shared__ float4 dp_dyn[];
+    __shared__ int s_cand[kDpMaxQ];             // the candidates' queries, ascending (torch.nonzero's order)
+    __shared__ float s_cscore[kDpMaxQ];         // and their max_score
+    __shared__ int s_order[kDpMaxQ];            // the candidates in score order, then the kept ones
+    __shared__ int s_wsum[kDpThreads / 32];
+    __shared__ float s_red[kDpThreads / 32];
+    __shared__ int s_n, s_K;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+    const float *bp = box_pred + (size_t)b * Q * 4;
+    const float *qm = qmax + (size_t)b * Q;
+    const int *qa = qarg + (size_t)b * Q;
+    const float mine = tid < Q ? qm[tid] : -INFINITY;
+    // block-wide compaction of the candidates in query order: ballot per warp, warp offsets from the warps' counts
+    const bool cand = tid < Q && mine > score_thres;
+    const unsigned ballot = __ballot_sync(0xffffffffu, cand);
+    if (lane == 0) s_wsum[tid >> 5] = __popc(ballot);
+    if (tid == 0) s_K = Q;
+    __syncthreads();
+    int base = 0;
+    for (int w = 0; w < (tid >> 5); ++w) base += s_wsum[w];
+    if (cand) {
+        const int at = base + __popc(ballot & ((1u << lane) - 1u));
+        s_cand[at] = tid;
+        s_cscore[at] = mine;
+    }
+    if (tid == kDpThreads - 1) s_n = base + s_wsum[tid >> 5];
+    __syncthreads();
+    const int n = s_n;
+    if (n == 0) {
+        // no candidate: the query of the largest max_score, the lowest one on exact ties (qmax is never NaN)
+        const float m = dp_block_max(mine, s_red);
+        if (tid < Q && mine == m) atomicMin(&s_K, tid);
+        __syncthreads();
+        if (tid == 0) { s_order[0] = s_K; s_K = 1; }
+    } else {
+        float4 *sbox = dp_dyn;
+        unsigned long long *mask = reinterpret_cast<unsigned long long *>(sbox + Q);
+        // batched_nms's coordinate trick on the candidates: m = boxes.max(), offset = class * (m + 1)
+        float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+        float m = -INFINITY;
+        if (tid < n) {
+            x = dp_xyxy(bp + 4 * s_cand[tid]);
+            m = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
+        }
+        m = dp_block_max(m, s_red);
+        const float m1 = __fadd_rn(m, 1.f);
+        // stable descending sort by rank counting over the candidates in query order
+        if (tid < n) {
+            const float si = s_cscore[tid];
+            int rank = 0;
+            for (int j = 0; j < n; ++j) {
+                const float sj = s_cscore[j];
+                rank += (sj > si || (sj == si && j < tid)) ? 1 : 0;
+            }
+            const int qi = s_cand[tid];
+            const float off = __fmul_rn((float)qa[qi], m1);
+            sbox[rank] = make_float4(__fadd_rn(x.x, off), __fadd_rn(x.y, off), __fadd_rn(x.z, off), __fadd_rn(x.w, off));
+            s_order[rank] = qi;
+        }
+        __syncthreads();
+        nms_bitmask<kDpThreads>(sbox, n, nms_iou, mask);
+        __syncthreads();
+        if (tid < 32) {
+            const int k = nms_sweep(mask, n, s_order);
+            if (tid == 0) s_K = k;
+        }
+    }
+    __syncthreads();
+    const int K = s_K;
+    // outputs in keep order; entries past K get detpost's fill values
+    const size_t o = (size_t)b * Q + tid;
+    if (tid < K) {
+        const int qi = s_order[tid];
+        scores[o] = qm[qi];
+        labels[o] = qa[qi];
+        query_index[o] = qi;
+        const float *src = bp + 4 * qi;
+        float4 box;
+        if (pixels) {                           // output_boxes[:, 0::2] *= W; output_boxes[:, 1::2] *= H; then to xyxy
+            const float sh = (float)ori_sizes[2 * b], sw = (float)ori_sizes[2 * b + 1];
+            box = dp_xyxy(__fmul_rn(__ldg(src), sw), __fmul_rn(__ldg(src + 1), sh), __fmul_rn(__ldg(src + 2), sw),
+                          __fmul_rn(__ldg(src + 3), sh));
+        } else {
+            box = make_float4(__ldg(src), __ldg(src + 1), __ldg(src + 2), __ldg(src + 3));
+        }
+        reinterpret_cast<float4 *>(boxes)[o] = box;
+    } else if (tid < Q) {
+        scores[o] = 0.f;
+        labels[o] = -1;
+        query_index[o] = -1;
+        reinterpret_cast<float4 *>(boxes)[o] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if (tid == 0) count[b] = K;
 }
 
 }  // namespace msda

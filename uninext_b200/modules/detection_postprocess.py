@@ -12,6 +12,9 @@ copy ``uninext_vid.py:1092-1197``):
 
 which synchronises with the host once per class and again for the NMS result.  ``postprocess_detections`` computes the
 same outputs without a host round trip, so it can be captured into a CUDA graph with the rest of a frame.
+
+``select_track_detections`` does the same for the video trackers' paths (``inference_mot`` and ``inference_vis`` of
+``uninext_vid.py``): score threshold, class-aware NMS and the kept queries, ready for ``tracker.match``.
 """
 from __future__ import annotations
 
@@ -22,8 +25,8 @@ import torch
 
 from uninext_b200 import _cabi
 
-MAX_QUERIES, MAX_TOKENS, MAX_CLASSES = 1024, 256, 4096      # include/msda_b200.h
-LAUNCHES = 2                                                  # per call, whatever B, Q, C and nms_iou
+MAX_QUERIES, MAX_TOKENS, MAX_CLASSES = 1024, 256, 4096      # include/msda_b200.h (and msda_trackpost.h)
+LAUNCHES = 2                                                  # per call, whatever B, Q, C and nms_iou (both entry points)
 
 
 class Detections(NamedTuple):
@@ -102,35 +105,14 @@ def postprocess_detections(box_cls: torch.Tensor, box_pred: torch.Tensor, positi
     CUDA graph is being captured are kept for the life of the process, so the graph's replays never read freed memory
     even after the cache has dropped them.
     """
-    if not (box_cls.is_cuda and box_pred.is_cuda and (iou_pred is None or iou_pred.is_cuda)):
-        raise RuntimeError("postprocess_detections: Not implemented on the CPU")
-    if box_cls.dim() != 3 or box_pred.shape != (*box_cls.shape[:2], 4):
-        raise ValueError(f"postprocess_detections: need box_cls [B, Q, T] and box_pred [B, Q, 4], got "
-                         f"{tuple(box_cls.shape)} and {tuple(box_pred.shape)}")
-    b, q, t = box_cls.shape
-    dev = box_cls.device
-    if iou_pred is not None:
-        if iou_pred.shape not in ((b, q, 1), (b, q)):
-            raise ValueError(f"postprocess_detections: iou_pred must be [B, Q, 1] or [B, Q], got {tuple(iou_pred.shape)}")
-        iou_pred = iou_pred.float().contiguous()
-    if not (1 <= q <= MAX_QUERIES and 1 <= t <= MAX_TOKENS):
-        raise ValueError(f"postprocess_detections: need 1 <= Q <= {MAX_QUERIES} and 1 <= T <= {MAX_TOKENS}, got Q={q}, T={t}")
+    b, q, t, dev, iou_pred = _check_inputs("postprocess_detections", box_cls, box_pred, iou_pred)
     class_start, tokens = positive_map_to_csr(positive_map, t, dev)
     c = class_start.numel() - 1
     k = int(max_num_inst)
     if not 1 <= k <= q * c:
         raise ValueError(f"postprocess_detections: need 1 <= max_num_inst <= Q*C = {q * c}, got {k}")
-    if isinstance(image_sizes, torch.Tensor):
-        if not image_sizes.is_cuda or image_sizes.shape != (b, 2):
-            raise ValueError("postprocess_detections: an image_sizes tensor must be a CUDA tensor [B, 2] (h, w)")
-        sizes = image_sizes.to(torch.int32).contiguous()
-    else:
-        sizes = _sizes(tuple((int(s[0]), int(s[1])) for s in image_sizes), dev)
-        if sizes.shape != (b, 2):
-            raise ValueError(f"postprocess_detections: {b} images but {sizes.shape[0]} image sizes")
-    if torch.cuda.is_current_stream_capturing():
-        for held in (class_start, tokens, sizes):
-            _CAPTURED[id(held)] = held
+    sizes = _device_sizes("postprocess_detections", "image_sizes", "image sizes", image_sizes, b, dev)
+    _hold_while_capturing(class_start, tokens, sizes)
     x = box_cls.float().contiguous()
     bx = box_pred.float().contiguous()
     ws_bytes = _cabi.workspace("msda_detpost_workspace", b, q, t, c, k)
@@ -143,3 +125,99 @@ def postprocess_detections(box_cls: torch.Tensor, box_pred: torch.Tensor, positi
                out.count, ws, ws.numel(), device=dev)
     return out
 
+
+def _check_inputs(fn: str, box_cls: torch.Tensor, box_pred: torch.Tensor, iou_pred: Optional[torch.Tensor]):
+    """(B, Q, T, device, iou_pred as contiguous fp32 or None) after the checks both entry points share."""
+    if not (box_cls.is_cuda and box_pred.is_cuda and (iou_pred is None or iou_pred.is_cuda)):
+        raise RuntimeError(f"{fn}: Not implemented on the CPU")
+    if box_cls.dim() != 3 or box_pred.shape != (*box_cls.shape[:2], 4):
+        raise ValueError(f"{fn}: need box_cls [B, Q, T] and box_pred [B, Q, 4], got "
+                         f"{tuple(box_cls.shape)} and {tuple(box_pred.shape)}")
+    b, q, t = box_cls.shape
+    if iou_pred is not None:
+        if iou_pred.shape not in ((b, q, 1), (b, q)):
+            raise ValueError(f"{fn}: iou_pred must be [B, Q, 1] or [B, Q], got {tuple(iou_pred.shape)}")
+        iou_pred = iou_pred.float().contiguous()
+    if not (1 <= q <= MAX_QUERIES and 1 <= t <= MAX_TOKENS):
+        raise ValueError(f"{fn}: need 1 <= Q <= {MAX_QUERIES} and 1 <= T <= {MAX_TOKENS}, got Q={q}, T={t}")
+    return b, q, t, box_cls.device, iou_pred
+
+
+def _device_sizes(fn: str, arg: str, what: str, sizes, b: int, dev: torch.device) -> torch.Tensor:
+    """B pairs (h, w) -> an int32 [B, 2] device tensor, cached per distinct content; a CUDA tensor [B, 2] as int32."""
+    if isinstance(sizes, torch.Tensor):
+        if not sizes.is_cuda or sizes.shape != (b, 2):
+            raise ValueError(f"{fn}: an {arg} tensor must be a CUDA tensor [B, 2] (h, w)")
+        return sizes.to(torch.int32).contiguous()
+    out = _sizes(tuple((int(s[0]), int(s[1])) for s in sizes), dev)
+    if out.shape != (b, 2):
+        raise ValueError(f"{fn}: {b} images but {out.shape[0]} {what}")
+    return out
+
+
+def _hold_while_capturing(*held: torch.Tensor) -> None:
+    """Keep cached device tensors that a CUDA graph being captured reads for the life of the process."""
+    if torch.cuda.is_current_stream_capturing():
+        for t in held:
+            _CAPTURED[id(t)] = t
+
+
+class TrackDetections(NamedTuple):
+    """``[B, Q]`` each (``boxes`` ``[B, Q, 4]``), ``count`` ``[B]``, in keep order.  Entries at and past ``count[b]``
+    hold the fill values: score 0, label -1, query_index -1, box 0."""
+    scores: torch.Tensor          # fp32 max over the classes (the reference's box_score), descending per frame
+    labels: torch.Tensor          # int32 argmax over the classes, 0-based (det_labels)
+    boxes: torch.Tensor           # fp32: xyxy in pixels of ori_size ("xyxy_pixels"), or normalised cxcywh ("cxcywh")
+    query_index: torch.Tensor     # int32 index into the Q queries: gathers pred_inst_embed and pred_masks
+    count: torch.Tensor           # int32 kept queries per frame, >= 1
+
+
+_BOX_FORMATS = {"cxcywh": _cabi.TRACKPOST_CXCYWH, "xyxy_pixels": _cabi.TRACKPOST_XYXY_PIXELS}
+
+
+def select_track_detections(box_cls: torch.Tensor, box_pred: torch.Tensor, positive_map: Dict[int, Sequence[int]],
+                            iou_pred: Optional[torch.Tensor] = None, *, score_thres: float, nms_iou: float,
+                            box_format: str, ori_sizes: Union[Sequence[Sequence[int]], torch.Tensor, None] = None
+                            ) -> TrackDetections:
+    """The per-frame detections the video trackers hand to ``tracker.match`` (``uninext_vid.py:1224-1250``
+    ``inference_mot``, ``:1380-1415`` ``inference_vis``), for B frames in two kernel launches
+    (``msda_trackpost_f32``, include/msda_trackpost.h) without a host round trip.
+
+    box_cls [B, Q, T] token logits, box_pred [B, Q, 4] normalised cxcywh, iou_pred [B, Q, 1] / [B, Q] or None,
+    positive_map = the reference's ``positive_map_label_to_token``.  Per frame: the class scores of
+    ``postprocess_detections``; ``max_score`` and ``label`` per query; the candidates ``max_score > score_thres`` in
+    query order; torchvision's ``batched_nms`` on them at ``nms_iou`` (0.7 for MOT, 0.9 for VIS); the kept queries in
+    keep order (score descending, ties to the lower query).  When no query passes the threshold, the result is the one
+    query of the largest ``max_score``, without NMS; on exact ties the lowest query, where the reference leaves the
+    choice to CPU ``topk``.  ``box_format="xyxy_pixels"`` gives MOT's ``det_bboxes[:, :4]``: each box scaled by
+    (W, H, W, H) of ``ori_sizes[b]`` = (h, w) (B pairs or an int32 CUDA tensor [B, 2]), then converted to xyxy.  The
+    reference scales ``pred_boxes`` in place; here the input is left as it is.  ``box_format="cxcywh"`` gives VIS's
+    normalised boxes unchanged.  Q <= 1024, T <= 256, C <= 4096.  Non-fp32 inputs are cast with ``.float()``.
+
+    The caller reads ``n = int(count[b])`` (the one host read per frame) and passes ``query_index[b, :n]``'s rows of
+    ``pred_inst_embed`` and ``pred_masks`` to the tracker (INTEGRATION.md section 6).
+    """
+    fn = "select_track_detections"
+    b, q, t, dev, iou_pred = _check_inputs(fn, box_cls, box_pred, iou_pred)
+    if box_format not in _BOX_FORMATS:
+        raise ValueError(f"{fn}: box_format must be one of {sorted(_BOX_FORMATS)}, got {box_format!r}")
+    class_start, tokens = positive_map_to_csr(positive_map, t, dev)
+    c = class_start.numel() - 1
+    sizes = None
+    if box_format == "xyxy_pixels":
+        if ori_sizes is None:
+            raise ValueError(f"{fn}: box_format='xyxy_pixels' needs ori_sizes")
+        sizes = _device_sizes(fn, "ori_sizes", "ori_sizes", ori_sizes, b, dev)
+    _hold_while_capturing(class_start, tokens, *(() if sizes is None else (sizes,)))
+    x = box_cls.float().contiguous()
+    bx = box_pred.float().contiguous()
+    ws_bytes = _cabi.workspace("msda_trackpost_workspace", b, q, t, c)
+    out = TrackDetections(torch.empty((b, q), dtype=torch.float32, device=dev),
+                          torch.empty((b, q), dtype=torch.int32, device=dev),
+                          torch.empty((b, q, 4), dtype=torch.float32, device=dev),
+                          torch.empty((b, q), dtype=torch.int32, device=dev), torch.empty((b,), dtype=torch.int32, device=dev))
+    ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=dev)
+    _cabi.call("msda_trackpost_f32", x, bx, iou_pred, class_start, tokens, sizes, b, q, t, c, float(score_thres),
+               float(nms_iou), _BOX_FORMATS[box_format], out.scores, out.labels, out.query_index, out.boxes, out.count,
+               ws, ws.numel(), device=dev)
+    return out
