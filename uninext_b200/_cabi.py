@@ -100,8 +100,15 @@ TRACKER_SIGNATURES = {
     "msda_idol_match_f32": (_i, [_vp] * 5 + [_i] * 5 + [ctypes.c_float] * 5 + [ctypes.c_double] + [_i] * 3 + [_vp] +
                             [_i] * 2 + [_vp] * 7 + [_vp, _i64, _vp]),
 }
+# And the QuasiDense tracker's (include/msda_qdtrack.h).
+QDTRACK_SIGNATURES = {
+    "msda_qdtrack_workspace": (_i, [_i] * 3 + [_vp]),
+    "msda_qdtrack_match_f32": (_i, [_vp] * 6 + [_i] * 3 + [ctypes.c_float] * 6 + [ctypes.c_double] + [_i] * 4 +
+                               [_vp] * 7 + [_vp, _i64, _vp]),
+}
 IDOL_LONG_MATCH, IDOL_FRAME_WEIGHT, IDOL_TEMPORAL_WEIGHT = 1, 2, 4                                # include/msda_tracker.h
 IDOL_OVERFLOW, IDOL_BAD_ROW = 1, 2
+QD_BACKDROPS, QD_MAX_BACKDROPS, QD_OVERFLOW, QD_BAD_ROW = 1, 1024, 1, 2                                  # include/msda_qdtrack.h
 TRACKPOST_CXCYWH, TRACKPOST_XYXY_PIXELS = 0, 1                                                         # include/msda_trackpost.h
 (KNOB_SLAB, KNOB_BWD_WIN_ROWS, KNOB_BWD_LIST_CAP, KNOB_FWD_SLAB_CTAS, KNOB_F32_VEC8_FWD, KNOB_F32_VEC8_BWD,
  KNOB_BF16_FINE_ROWS, KNOB_BF16_PACKED_FWD, KNOB_ZERO_FILL, KNOB_REGION_BWD) = range(10)                                                   # include/msda_b200.h
@@ -156,7 +163,7 @@ def entry(name: str, path: str | None = None):
     fn = _entries.get(name) if path is None else None
     if fn is None:
         lib = load(path)
-        late = TRACKPOST_SIGNATURES.get(name) or TRACKER_SIGNATURES.get(name)
+        late = TRACKPOST_SIGNATURES.get(name) or TRACKER_SIGNATURES.get(name) or QDTRACK_SIGNATURES.get(name)
         if name in lib.missing or (late and not hasattr(lib, name)):
             raise MSDALibraryError(f"{path or LIB_PATH} does not export `{name}` (stale build? run "
                                    "uninext_b200.build --force)")
@@ -192,6 +199,11 @@ def trackpost(path: str | None = None):
 def tracker(path: str | None = None):
     """The library, after checking that it exports the IDOL tracker's association step (include/msda_tracker.h)."""
     return _with_group(TRACKER_SIGNATURES, path)
+
+
+def qdtrack(path: str | None = None):
+    """The library, after checking that it exports the QuasiDense tracker's association step (include/msda_qdtrack.h)."""
+    return _with_group(QDTRACK_SIGNATURES, path)
 
 
 def call(name: str, *args, device) -> None:

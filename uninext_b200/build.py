@@ -23,7 +23,7 @@ INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include")
 SOURCES = ["msda_cabi.cu", "msda_cabi_module.cu", "msda_cabi_condinst.cu", "msda_cabi_postprocess.cu", "msda_cabi_vlfuse.cu",
            "msda_cabi_twostage.cu", "msda_cabi_flatten.cu", "msda_cabi_tracker.cu", "msda_gemm_sm90.cu"]
 HEADERS = ["msda_host.cuh", "msda_common.cuh", "msda_tiled.cuh", "msda_region.cuh", "msda_slab.cuh", "msda_tmem.cuh", "msda_generic.cuh", "msda_module.cuh", "msda_condinst.cuh", "msda_maskpaste.cuh", "msda_maskrle.cuh","msda_detpost.cuh", "msda_det.cuh", "msda_vlfuse.cuh", "msda_vlfuse_tc.cuh", "msda_layernorm.cuh", "msda_topk.cuh",
-           "msda_twostage.cuh", "msda_flatten.cuh", "msda_nms.cuh", "msda_tracker.cuh"]
+           "msda_twostage.cuh", "msda_flatten.cuh", "msda_nms.cuh", "msda_tracker.cuh", "msda_qdtrack.cuh"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -45,7 +45,7 @@ def is_stale() -> bool:
     if not os.path.exists(LIB_PATH):
         return True
     built = os.path.getmtime(LIB_PATH)
-    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.join(INCLUDE, h) for h in ("msda_b200.h", "msda_twostage.h", "msda_flatten.h", "msda_trackpost.h", "msda_tracker.h")] + [__file__]
+    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.join(INCLUDE, h) for h in ("msda_b200.h", "msda_twostage.h", "msda_flatten.h", "msda_trackpost.h", "msda_tracker.h", "msda_qdtrack.h")] + [__file__]
     return any(os.path.exists(d) and os.path.getmtime(d) > built for d in deps)
 
 

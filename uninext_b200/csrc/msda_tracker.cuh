@@ -25,6 +25,12 @@ struct IdolParams {
     int frame_weight, memo_frames, frame_id, long_match, L;
 };
 
+// The momentum update of a tracklet's embedding, (1 - m) * old + m * x as torch evaluates it on fp32 tensors: the two
+// weights rounded to fp32, each product and the sum rounded once.  Shared by both trackers.
+__device__ __forceinline__ float tracker_ema(float keep_w, float old, float new_w, float x) {
+    return __fadd_rn(__fmul_rn(keep_w, old), __fmul_rn(new_w, x));
+}
+
 // torch's CUDA sigmoid (1 / (1 + exp(-x)) in fp32, IEEE division) compared with 0.5, as the reference binarises.
 __device__ __forceinline__ bool idol_on(float x) { return 1.0f / (1.0f + expf(-x)) > 0.5f; }
 
@@ -174,15 +180,17 @@ __global__ void __launch_bounds__(kIdolThreads) idol_memo(const int *__restrict_
     }
 }
 
-// feats[i, c] = E[rows[kept[i]]] . M[c] for i < k, c < live, fp32, in 32 x 32 tiles (row stride T).
+// feats[i, c] = E[rows[kept[i]]] . M[c] for i < k, c < live = *cols, fp32, in 32 x 32 tiles (row stride T).  Nothing
+// when the error word *err is set.  Shared by both trackers (msda_qdtrack.cuh).
 __global__ void __launch_bounds__(kIdolThreads) idol_feats(const float *__restrict__ embeds, const int *__restrict__ rows,
                                                            const int *__restrict__ kept, const int *__restrict__ kept_count,
-                                                           const int *__restrict__ state, const float *__restrict__ M,
-                                                           int T, int D, float *__restrict__ F)
+                                                           const int *__restrict__ cols, const int *__restrict__ err,
+                                                           const float *__restrict__ M, int T, int D,
+                                                           float *__restrict__ F)
 {
-    const int k = *kept_count, live = state[0];
+    const int k = *kept_count, live = *cols;
     const int i0 = blockIdx.y * kIdolTile, c0 = blockIdx.x * kIdolTile, t = threadIdx.x;
-    if (i0 >= k || c0 >= live || state[2]) return;
+    if (i0 >= k || c0 >= live || *err) return;
     __shared__ float sa[kIdolTile][kIdolTile + 1], sb[kIdolTile][kIdolTile + 1];
     __shared__ const float *arow[kIdolTile];
     if (t < kIdolTile) arow[t] = i0 + t < k ? embeds + (size_t)rows[kept[i0 + t]] * D : nullptr;
@@ -235,16 +243,18 @@ __device__ __forceinline__ float idol_block_sum(float v, float *red) {
     return v;
 }
 
-// CTAs 0 .. n_cap - 1: row i's max and sum of exp(f - max) over the live columns (softmax over the memo); CTAs n_cap + c:
-// column c's over the kept rows (softmax over the detections).  stat[2 x] = (max, sum).
+// CTAs 0 .. n_cap - 1: row i's max and sum of exp(f - max) over the live = *cols columns (softmax over the memo); CTAs
+// n_cap + c: column c's over the kept rows (softmax over the detections).  stat[2 x] = (max, sum).  Nothing when the
+// error word *err is set.  Shared by both trackers.
 __global__ void __launch_bounds__(kIdolThreads) idol_softmax_stats(const float *__restrict__ F,
                                                                    const int *__restrict__ kept_count,
-                                                                   const int *__restrict__ state, int n_cap, int T,
+                                                                   const int *__restrict__ cols,
+                                                                   const int *__restrict__ err, int n_cap, int T,
                                                                    float *__restrict__ rstat, float *__restrict__ cstat)
 {
     __shared__ float red[kIdolThreads / 32];
-    const int k = *kept_count, live = state[0], b = blockIdx.x;
-    if (state[2]) return;
+    const int k = *kept_count, live = *cols, b = blockIdx.x;
+    if (*err) return;
     const bool row = b < n_cap;
     const int x = row ? b : b - n_cap, len = row ? live : k;
     if (x >= (row ? k : live) || len == 0) return;
@@ -449,7 +459,7 @@ __global__ void __launch_bounds__(kIdolThreads) idol_update(const float *__restr
     float *em = embed + (size_t)slot * D, *re = ring_e + (size_t)slot * L * D, *rsc = ring_s + (size_t)slot * L;
     for (int d = threadIdx.x; d < D; d += kIdolThreads) {
         const float x = e[d];
-        em[d] = fresh ? x : __fadd_rn(__fmul_rn(p.keep_w, em[d]), __fmul_rn(p.new_w, x));
+        em[d] = fresh ? x : tracker_ema(p.keep_w, em[d], p.new_w, x);
         if (len < L) {
             re[(size_t)len * D + d] = x;
         } else {
